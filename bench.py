@@ -12,11 +12,15 @@ is evaluated, replies and new AppendEntries are emitted for the next step.
  e2e        the same flood driven through the public C ABI (ra_engine_step with pinned HOST
             buffers; H2D of the step's events and D2H of its notes inside every step).
  roofline   algorithmic bytes (SURVEY.md §8d: B_commit(5) = 2884 B, B_commit(7) = 4282 B per
-            committed entry) / duration of the raft_step launches / measured HBM peak.
+            committed entry) / duration of the raft_step launches / HBM peak (MEASURED_PEAKS.json
+            when present, else the H100 SXM data-sheet 3.35 TB/s).
  cpu_baseline  the CPU restatement of ra_server (oracle/, kind "port": the reference is Erlang
             and no OTP toolchain exists on the box) on a bounded sample of the same workload.
 
  --impl reference times that CPU port with all host threads (see DESIGN.md "reference arm").
+ --dump-outputs DIR  after the timed steps, writes what the timed flood left for its caller (a fixed
+            sample of the member rows, every ra_row_state field, and the counters) as float64 .npy files,
+            so that two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -30,30 +34,14 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True          # the benchmark leaves the tree as it found it (it may be read-only)
 
 B_COMMIT = {3: 40 + 104 * 3 + 2 * (169 + 185) + (128 + 8 * 3) + 2 * (145 + 8 * 3),
             5: 2884, 7: 4282}
 METRIC = "committed entries/sec across N Raft groups; HBM GB/s vs roofline"
-# dram__bytes_read.sum + dram__bytes_write.sum of raft_step_kernel per launch: read from the committed ncu summary
-# of the shipped build (tools/ncu_summary.py output of one `ncu --set full` capture of this workload)
-TRAFFIC_FILE = os.path.join(ROOT, "profiles", "r02_raft_step_ncu_full.txt")
-
-
-def traffic_bytes():
-    """-> (bytes per launch or None, source)"""
-    try:
-        rd = wr = None
-        for ln in open(TRAFFIC_FILE):
-            f = ln.split()
-            if len(f) >= 3 and f[0] == "dram__bytes_read.sum":
-                rd = float(f[1]) * {"[Mbyte]": 1e6, "[Gbyte]": 1e9, "[Kbyte]": 1e3, "[byte]": 1.0}[f[2]]
-            if len(f) >= 3 and f[0] == "dram__bytes_write.sum":
-                wr = float(f[1]) * {"[Mbyte]": 1e6, "[Gbyte]": 1e9, "[Kbyte]": 1e3, "[byte]": 1.0}[f[2]]
-        if rd is not None and wr is not None:
-            return int(rd + wr), os.path.relpath(TRAFFIC_FILE, ROOT)
-    except (OSError, KeyError, ValueError):
-        pass
-    return None, "no ncu summary found"
+HBM_NOMINAL_GBS = 3350.0                # H100 SXM data sheet, HBM3
+L2_BYTES = 50e6                         # H100 SXM
+DUMP_ROWS = 1 << 15                     # --dump-outputs: member rows sampled (84 float64 each: 22 MB)
 
 
 def b_commit(m: int) -> int:
@@ -66,7 +54,49 @@ def hbm_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return HBM_NOMINAL_GBS, "nominal (H100 SXM data sheet)"
+
+
+def gpu_info(dev: int) -> dict:
+    """The card a number was measured on: its name, power limit and top SM clock."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(dev)}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(dev), "--query-gpu=power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        pl, mx = (x.strip() for x in r.stdout.strip().split(",")[:2])
+        out["power_limit_w"], out["sm_max_mhz"] = float(pl), float(mx)
+    except Exception:
+        out["power_limit_w"] = None
+    return out
+
+
+def _row_vector(r) -> list:
+    """One ra_row_state as a fixed-length vector of the fields the parity diff compares (key()); the runs past
+    n_runs, the peers past n_members and an invalid await_condition reply are zeros."""
+    from ra_b200 import abi
+    k = r.key()
+    starts, terms, cond, peers = k[24], k[25], k[26], k[27]
+    v = list(k[:24])
+    v += list(starts) + [0] * (abi.RA_MAX_RUNS - len(starts))
+    v += list(terms) + [0] * (abi.RA_MAX_RUNS - len(terms))
+    v += list(cond) if cond else [0] * 4
+    for p in range(abi.RA_MAX_MEMBERS):
+        v += list(peers[p]) if p < len(peers) else [0] * 5
+    return v
+
+
+def dump_outputs(out_dir: str, eng, counters: dict, prefix: str = "") -> None:
+    """What a caller of the timed flood receives once it ends: the member rows (ra_engine_read_rows) -- all of
+    them, or a fixed, seeded sample of DUMP_ROWS -- and the counters (ra_engine_counters), as float64 arrays."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = eng.n_rows
+    ids = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+    rows = np.array([_row_vector(r) for r in eng.read_rows(ids.tolist())], dtype=np.float64)
+    np.save(os.path.join(out_dir, prefix + "row_ids.npy"), ids.astype(np.float64))
+    np.save(os.path.join(out_dir, prefix + "rows.npy"), rows)
+    np.save(os.path.join(out_dir, prefix + "counters.npy"), np.array(list(counters.values()), dtype=np.float64))
 
 
 class ClockSampler:
@@ -270,6 +300,8 @@ def run_engine(args):
     barrier_sync(world, local)
     clocks = sampler.stop()
     c1 = eng.counters()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, eng, c1, prefix="rank%d_" % rank if world > 1 else "")
     commits = c1["commits"] - c0["commits"]
     events = c1["events"] - c0["events"]
     dropped = c1["msgs_dropped"] - c0["msgs_dropped"]
@@ -370,7 +402,6 @@ def run_engine(args):
     if rank != 0:
         return
     peak, peak_src = hbm_peak()
-    traffic, traffic_src = traffic_bytes()
     bc = b_commit(M)
     achieved = (commits / (ms * 1e-3)) * bc / 1e9               # this rank, GB/s
     par = ("members of a group on different GPUs ((group+slot) mod N); " +
@@ -392,13 +423,12 @@ def run_engine(args):
                 "events_per_step": events_all / args.steps, "commits_per_step": commits_all / args.steps,
                 "msgs_dropped": dropped},
         "gpu_launches": launches,
+        "gpu": gpu_info(dev),
         "clocks": clocks,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                     # SURVEY 8d: also against the nominal HBM3e figure; and what the kernel really moves
-                     "peak_nominal": 8000.0, "frac_nominal": achieved / 8000.0,
-                     "achieved_traffic": (traffic / 1e9) / (ms * 1e-3 / args.steps) if (traffic and world == 1 and args.config == 3) else None,
-                     "frac_traffic": ((traffic / 1e9) / (ms * 1e-3 / args.steps) / peak) if (traffic and world == 1 and args.config == 3) else None,
+                     "frac": achieved / peak, "peak_source": peak_src,
+                     # SURVEY 8d: also against the nominal HBM3 figure
+                     "peak_nominal": HBM_NOMINAL_GBS, "frac_nominal": achieved / HBM_NOMINAL_GBS,
                      "bytes_per_commit": bc, "algorithmic_bytes_per_launch": bc * commits / args.steps,
                      "kernel": "raft_step_kernel (+ raft_general_kernel for the rows that leave the fast paths)"},
     }
@@ -537,8 +567,8 @@ def workload_config(args) -> dict:
                         % (G, M, args.cmds, args.permille / 10.0, args.config - 1,
                            (", faults %s" % (args.faults,)) if args.faults else ""),
             "groups_per_gpu": G, "members": M, "cmds_per_step": args.cmds, "election_permille": args.permille,
-            "l2": "working set (SoA %.0f MB + mailboxes) %s the 126 MB L2; no explicit flush"
-                  % (G * M * 392 / 1e6, "exceeds" if G * M * 392 > 126e6 else "fits in")}
+            "l2": "working set (SoA %.0f MB + mailboxes) %s the %.0f MB L2; no explicit flush"
+                  % (G * M * 392 / 1e6, "exceeds" if G * M * 392 > L2_BYTES else "fits in", L2_BYTES / 1e6)}
 
 
 def parity_sample(args, eng, world: int, rank: int, spread: bool, seed: int, flood_steps: int, stride: int = 97) -> dict:
@@ -702,6 +732,9 @@ def main():
                     help="skip the keyed entries for the other configs (N=1: 2, 4, 5; N>1: 4 strong-scaled)")
     ap.add_argument("--no-latency", dest="latency", action="store_false", help="skip the per-call latency probe (N=1)")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle replay of every 97th group of this run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the member rows (a fixed sample of %d when there are more) and "
+                         "the counters the timed flood left as float64 .npy files under DIR" % DUMP_ROWS)
     args = ap.parse_args()
     args.faults = None
     if args.config != 3:

@@ -1,5 +1,5 @@
 /*
- * ra_engine.h -- C ABI of the B200 batched multi-Raft engine.
+ * ra_engine.h -- C ABI of the H100 batched multi-Raft engine.
  *
  * Drop-in boundary: the call from ra_server_proc into the pure Raft core,
  *   ra_server:handle_leader(Msg, State)            src/ra_server_proc.erl:1354

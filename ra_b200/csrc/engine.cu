@@ -1,4 +1,4 @@
-// engine.cu -- C ABI (include/ra_engine.h) of the B200 batched multi-Raft engine.
+// engine.cu -- C ABI (include/ra_engine.h) of the H100 batched multi-Raft engine.
 //
 // Host side: owns the HBM Struct-of-Arrays, stages host buffers, launches per step
 //   raft_step_kernel     -- the hot path: one thread per member row, steady-state fast paths
@@ -27,11 +27,11 @@
 #endif
 #ifndef MINB
 #define MINB 5                              // CTAs per SM the register allocation is held to: 20 warps,
-                                            // <= 96 registers (no spills), 5 x 39 KB of shared memory
+                                            // <= 96 registers, 5 x 39 KB of the SM's 228 KB of shared memory
 #endif
 #ifndef MINB_NARROW
-#define MINB_NARROW 5                       // the narrow pass (32-bit index arithmetic) needs ~84 registers: measured
-#endif                                      // 0.0796 ms at 5 CTAs/SM (no spill), 0.0816 at 6 (80 regs, 24 B), 0.0865 at 7 (72, 68 B)
+#define MINB_NARROW 5                       // the narrow pass (32-bit index arithmetic) fits 96 registers without
+#endif                                      // spilling at 5 CTAs/SM; at 6 it spills and is slower (DESIGN.md §4)
 #define TILE_BYTES (RT * 64)
 #define RA_BAR_WORDS 64                       // barrier flag words behind mbox_cnt[b] (one per source shard)
 #define WARPS (CTA_T / 32)
@@ -40,7 +40,7 @@
 #define RA_N_COUNTERS (8 + 8 * 16 + 8)
 #define RA_CNT_REF 136
 
-// ---- TMA (cp.async.bulk) + mbarrier, sm_90+/sm_100a --------------------------------------
+// ---- TMA (cp.async.bulk) + mbarrier, sm_90a ------------------------------------------------
 __device__ __forceinline__ u32 smem_u32(const void* p) { return (u32)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(u64* bar, u32 count)
 { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count)); }
@@ -742,7 +742,7 @@ extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
 #undef SMEM_ATTR
 #undef SMEM_ATTR_NS
     {
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
         e->general_grid = (u32)sms * 2;
     }

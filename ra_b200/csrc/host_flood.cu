@@ -114,7 +114,7 @@ extern "C" int ra_hostsim_create_multi(ra_engine* const* engines, uint32_t n, ra
         s->threads = env ? (u32)atoi(env) : (hc > 16 ? 16u : (hc ? hc : 1u));
         if (s->threads < 1) s->threads = 1;
         const char* de = getenv("RA_HOSTSIM_DRIVERS");
-        u32 nd = de ? (u32)atoi(de) : 1u;      // measured: the flood is PCIe-bound from 4 partitions on, a second driver adds nothing
+        u32 nd = de ? (u32)atoi(de) : 1u;      // one driver: the host model's threads, not the driver's waits, bound the flood
         if (nd < 1) nd = 1;
         if (nd > n) nd = n;
         s->drivers.resize(nd);

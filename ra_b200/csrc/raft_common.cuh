@@ -1,4 +1,4 @@
-// raft_common.cuh -- device side of the batched multi-Raft engine (sm_100a): what both passes of the logic share
+// raft_common.cuh -- device side of the batched multi-Raft engine (sm_90a): what both passes of the logic share
 // (raft_step.cuh includes raft_logic.cuh / raft_row_logic.cuh twice: 64-bit and 32-bit index arithmetic).
 //
 // One thread owns one member row for the whole launch ("owner computes"): every HBM column

@@ -25,7 +25,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(_SO):
             raise EngineUnavailable(
                 "%s is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). The engine has no CPU fallback." % _SO)
+                "(nvcc, sm_90a). The engine has no CPU fallback." % _SO)
         _lib = C.CDLL(_SO)
         _lib.ra_engine_flood.restype = C.c_int
         _lib.ra_engine_flood.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]

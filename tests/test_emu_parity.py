@@ -3,7 +3,7 @@ host by tests/emu/) against the oracle, with the inputs of the `-m gpu` parity t
 
 What this covers: every handler / fast path / codec / end-of-step line the GPU executes, driven
 with the control flow of the two step kernels.  What it does not: the kernels' own frame (TMA
-ring, warp reductions, launches) -- tests/test_parity_gpu.py does that on a B200.
+ring, warp reductions, launches) -- tests/test_parity_gpu.py does that on an H100.
 """
 import ctypes as C
 

@@ -28,8 +28,8 @@ def test_nccl_sharded_flood_equals_oracle(world, transport, tmp_path):
     import torch
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    # round 1: verified on B200 boxes at world 2 and 4 (both transports); at world 8 the bucket
-    # transport failed its first run (log lost, bucket capacity raised since) -- see DESIGN.md §7
+    # at world 8 > M = 5 two slot offsets share one destination shard: the bucket capacity of
+    # sharded.Shard must cover that, or records are dropped and the rows differ -- see DESIGN.md §8
     script = tmp_path / "w.py"
     script.write_text(textwrap.dedent("""
         import os, sys

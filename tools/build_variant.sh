@@ -4,6 +4,6 @@
 set -e
 v=$1; shift
 cd "$(dirname "$0")/../ra_b200/csrc"
-/usr/local/cuda/bin/nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-fopenmp -Xptxas -v \
+/usr/local/cuda/bin/nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp -Xptxas -v \
   "$@" -shared -o libra_engine_$v.so engine.cu host_flood.cu -lgomp 2> build_$v.log || { cat build_$v.log; exit 1; }
 grep -A3 "Compiling entry function '_Z16raft_step_kernelILi261" build_$v.log | grep -E "Used|spill" | tr '\n' ' '; echo " [$v $*]"
