@@ -23,7 +23,7 @@
 // the hot kernel
 // ------------------------------------------------------------------------------------------
 #ifndef NST
-#define NST 3                               // shared-memory stages per warp: NST record tiles (1 or 2 KB) in flight
+#define NST 3                               // shared-memory stages per warp: NST record tiles (0.5, 1 or 2 KB) in flight
 #endif
 #ifndef MINB
 #define MINB 5                              // CTAs per SM the register allocation is held to: 20 warps,
@@ -183,7 +183,7 @@ raft_general_kernel(const __grid_constant__ Cols C, const int cur, const FloodAr
             m.lrs_ok = 0;
             m.n_msgs = (u32)q1.x & 0xffffu; m.n_notes = ((u32)q1.x >> 16) & 0xffffu; m.status = (u32)(q1.x >> 32);
             m.sent_to = (u32)q1.y;
-            { const u32 w = (u32)(q1.y >> 32); m.pn_type = w & 0xffu; m.pn_slot = (w >> 8) & 0xffu; m.wk = w >> 16; }
+            { const u32 w = (u32)(q1.y >> 32); m.pn_type = w & 0xffu; m.pn_slot = (w >> 8) & 0xffu; m.wk = (w >> 16) | ((u32)q3.y << 16); }
             m.pn_a = q2.x; m.pn_b = q2.y; m.pn_c = q3.x;
             u64 big = 0;                                        // see row_mark_wide
             if (flags & STALL_PENDING) {
@@ -270,13 +270,15 @@ __global__ void ingest_kernel(const Cols C, const ra_event* ev, u32 n, u32* err,
     while (i + len < n && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
     if (len > RA_LOCAL_CAP) { atomicMax(err, 2u); return; }
     if (atomicCAS(&C.loc_n[row], 0u, len) != 0u) { atomicMax(err, 1u); return; }
-    u32 tails = 0;
-    for (u32 k = 0; k < len; k++)
-        if (st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]))) tails |= 0x100u << k;
-    if (tails) atomicOr(&C.loc_n[row], tails);
+    u32 size = 0;                                              // loc_n bits 8 + k (tail), 12 + k (not short)
+    for (u32 k = 0; k < len; k++) {
+        const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]));
+        size |= (((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12)) << k;
+    }
+    if (size) atomicOr(&C.loc_n[row], size);
 }
 
-// the same for a batch of 32-byte host events: every record is a head (RS_PLAIN); err 3 also for an RPC type
+// the same for a batch of 32-byte host events: every record is RS_PLAIN; err 3 also for an RPC type
 __device__ __forceinline__ bool host_event_type_ok(u32 t)
 {
     return t == RA_EV_WRITTEN || t == RA_EV_COMMAND || t == RA_EV_ELECTION_TIMEOUT || t == RA_EV_AWAIT_COND_TIMEOUT ||
@@ -293,14 +295,14 @@ __global__ void ingest_host_kernel(const Cols C, const ra_host_event* ev, u32 n,
     while (i + len < n && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
     if (len > RA_LOCAL_CAP) { atomicMax(err, 2u); return; }
     if (atomicCAS(&C.loc_n[row], 0u, len) != 0u) { atomicMax(err, 1u); return; }
+    u32 heads = 0;
     for (u32 k = 0; k < len; k++) {
         const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&ev[i + k]);
         const ulonglong2 h = src[0], t = src[1];               // {row | type<<32 | flags<<40 | n<<48, term}, {a, b}
-        ulonglong2* q = C.loc + rec_word(C.tiles, k, row, 0);
-        const u64 type = (h.x >> 32) & 0xffull, flags = (h.x >> 40) & 0xffull, nn = (h.x >> 48) & 0xffffull;
-        q[0] = make_ulonglong2(type | ((u64)RA_NO_SLOT << 8) | (flags << 16) | ((u64)RS_PLAIN << 24) | (nn << 32), h.y);
-        q[RT] = t;
+        const u32 type = (u32)(h.x >> 32) & 0xffu, flags = (u32)(h.x >> 40) & 0xffu, nn = (u32)(h.x >> 48);
+        heads |= put_local(C.loc, C.tiles, k, row, type, flags, nn, h.y, t.x, t.y) << (12 + k);
     }
+    if (heads) atomicOr(&C.loc_n[row], heads);
 }
 
 // records that other shards sent to members of this engine -> mailbox planes of the next step.

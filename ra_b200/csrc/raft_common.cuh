@@ -157,6 +157,10 @@ struct StallCtx {                      // 4 x 16 bytes
     u32 row, flags, rem_mbox, rem_loc;
     u32 n_msgs_notes, status, sent_to, pn_type_slot_wk;
     u64 pn_a, pn_b;
-    u64 pn_c, _pad;
+    u64 pn_c;
+    // Member::wk >> 16 -- the per-peer "sent a record that is not short" bits; pn_type_slot_wk keeps its low 16 bits.
+    // (_pad is the name the host emulation knows this word by: it stores 0 there, which is exact for it because its
+    // readers decode every record from the record's own chunk 0 and never use the size flags of the counts.)
+    union { u64 wk_hi; u64 _pad; };
 };
 #define STALL_PENDING 1u               // the deferred pipeline pass has not run yet

@@ -10,7 +10,8 @@
 // everything that ever writes the row (load_rows, both kernels), means that every value of its state is below 2^30
 // plus what one step can add -- and (b) every field of the record at hand is below 2^30 (rec_decode says so);
 // anything else stalls to raft_general_kernel, which computes on the ABI's 64 bits.  Memory formats are the same
-// in both passes (64-bit cells, 64-byte records): W() widens on the way out, N() narrows on the way in.
+// in both passes (64-bit cells; records in the planes as 16-byte short, 32-byte head or 64-byte long form, see
+// "record planes" below): W() widens on the way out, N() narrows on the way in.
 #if RA_NARROW_PASS
 typedef u32 ix_t;
 typedef int sx_t;
@@ -52,20 +53,59 @@ __device__ __forceinline__ void st_rec(ra_event* p, const Rec& r)
     ulonglong2* q = reinterpret_cast<ulonglong2*>(p);
     q[0] = r.w0; q[1] = r.w1; q[2] = r.w2; q[3] = r.w3;
 }
-// ---- record planes: 32-byte head + optional 32-byte tail ---------------------------------------
-// Inside the engine (mailbox and host-event planes) a record is stored as
-//   chunk 0 {H, term}   chunk 1 {x, y}   [chunk 2 {c, d}   chunk 3 {e, -}]
-//   H = type | from << 8 | flags << 16 | shape << 24 | dbit << 31 | n << 32 | n1 << 48
+#endif
+// ---- record planes: 16-byte short form, 32-byte head, optional 32-byte tail ------------------------
+// Inside the engine (mailbox and host-event planes) a record is stored in one of three forms:
+//   short  chunk 0 {S | term << 32, x | y << 32}
+//          S = type | from << 4 | flags << 8 | shape << 12 | n << 14 | n1 << 22 | 1 << 30 | dbit << 31
+//          (4-bit from: slot 0..7, 15 = RA_NO_SLOT)
+//   head   chunk 0 {H, term}   chunk 1 {x, y}
+//          H = type | from << 8 | flags << 16 | shape << 24 | dbit << 31 | n << 32 | n1 << 48
+//   long   the head + chunk 2 {c, d}   chunk 3 {e, -}   (shape RS_LONG)
+// Bits 26..30 of H are always zero, so bit 30 of chunk 0 (RS_SHORT) tells the short form from the others.
 // The shape says how a..e are rebuilt -- a lossless re-encoding that does not depend on the type:
 //   RS_LONG   a = x, b = y, c d e from the tail
 //   RS_PLAIN  a = x, b = y, c = d = e = 0                       written, command, vote requests ...
 //   RS_REPLY  a = x, b = y, c = term, d = dbit, e = 0           append_entries_reply in steady state
 //   RS_AER    a = x, b = term, c = y, d = dbit ? term : 0, e = 0  append_entries_rpc in steady state
-// Chunks 0 and 1 of a tile are contiguous (1 KB), so a tile none of whose records has a tail costs
-// half the bytes to write and to fetch; whether a tail exists travels with the record counts
-// (bit 3 of the per-sender count nibble / bits 8.. of loc_n).
+// A record is written short when its shape is not RS_LONG, term, x and y are below 2^32, type and flags below
+// 16, from a slot 0..7 or RA_NO_SLOT and n, n1 below 256: every steady-state record.  Chunks 0..3 of a tile are
+// contiguous 512-byte blocks, so a tile all of whose records are short costs a quarter of the bytes of a long
+// one to write and to fetch, a tile without a tail half.  What the records of a tile need travels with the
+// record counts: bit 3 (some record has a tail) and bit 4 (some record is not short) of the per-sender count
+// byte; bits 8..11 (tail) and 12..15 (not short) of loc_n, one per host slot.  A reader never looks past
+// chunk 0 of a short record: in the hot kernel's staging slot the other chunks hold an earlier tile's bytes.
 enum { RS_LONG = 0, RS_PLAIN = 1, RS_REPLY = 2, RS_AER = 3 };
-__device__ __forceinline__ bool st_rec_plane(ulonglong2* base, u32 tiles, u32 plane, u32 row, const Rec& r)
+#define RS_SHORT 0x40000000u                                    // bit 30 of chunk 0: the short form
+enum { RF_NOT_SHORT = 1, RF_TAIL = 2 };                         // what st_rec_plane wrote besides chunk 0
+#if defined(RA_HOST_EMU) && defined(RA_PLANE_STATS)
+// test observability (a host build of the emulation with RA_PLANE_STATS, tests/emu/plane_stats.cpp): every record
+// stored into a plane, by type and form (0 short, 1 head, 3 long)
+extern "C" void ra_emu_plane_store(unsigned type, unsigned form);
+#endif
+__device__ __forceinline__ u32 plane_stored(u32 type, u32 form)
+{
+#if defined(RA_HOST_EMU) && defined(RA_PLANE_STATS)
+    ra_emu_plane_store(type, form);
+#endif
+    return form;
+}
+__device__ __forceinline__ bool rec_short_fits(u32 type, u32 from, u32 flags, u32 n, u32 n1)
+{ return type < 16u && (from < 8u || from == RA_NO_SLOT) && flags < 16u && (n | n1) < 256u; }
+__device__ __forceinline__ u32 rec_short_hdr(u32 type, u32 from, u32 flags, u32 shape, u32 dbit, u32 n, u32 n1)
+{ return type | ((from & 15u) << 4) | (flags << 8) | (shape << 12) | (n << 14) | (n1 << 22) | RS_SHORT | (dbit << 31); }
+__device__ __forceinline__ bool rec_is_short(const ulonglong2& c0) { return ((u32)c0.x & RS_SHORT) != 0; }
+__device__ __forceinline__ bool rec_has_tail(const ulonglong2& c0) { return ((u32)c0.x & (RS_SHORT | (3u << 24))) == (RS_LONG << 24); }
+// the head word H (low 32 bits | n | n1 << 16 as the high 32) of a short record's S
+__device__ __forceinline__ u32 short_hlo(u32 S)
+{
+    const u32 f = (S >> 4) & 15u;
+    return (S & 15u) | ((f == 15u ? RA_NO_SLOT : f) << 8) | (((S >> 8) & 15u) << 16) | (((S >> 12) & 3u) << 24) | (S & 0x80000000u);
+}
+__device__ __forceinline__ u32 short_nn(u32 S) { return ((S >> 14) & 0xffu) | (((S >> 22) & 0xffu) << 16); }
+
+#if !RA_NARROW_PASS
+__device__ __forceinline__ u32 st_rec_plane(ulonglong2* base, u32 tiles, u32 plane, u32 row, const Rec& r)
 {
     const u64 term = r.w1.x, a = r.w1.y, b = r.w2.x, c = r.w2.y, d = r.w3.x, e = r.w3.y;
     u32 shape = RS_LONG, dbit = 0;
@@ -75,25 +115,35 @@ __device__ __forceinline__ bool st_rec_plane(ulonglong2* base, u32 tiles, u32 pl
         else if (c == term && d <= 1) { shape = RS_REPLY; dbit = (u32)d; }
         else if (b == term && (d == 0 || d == term)) { shape = RS_AER; y = c; dbit = d != 0; }
     }
-    const u64 H = ((r.w0.x >> 32) & 0x00FFFFFFull) | ((u64)shape << 24) | ((u64)dbit << 31) | (r.w0.y << 32);
+    const u32 hd = (u32)(r.w0.x >> 32), type = hd & 0xffu, from = (hd >> 8) & 0xffu, flags = (hd >> 16) & 0xffu;
+    const u32 n = (u32)r.w0.y & 0xffffu, n1 = (u32)(r.w0.y >> 16) & 0xffffu;
     ulonglong2* q = base + rec_word(tiles, plane, row, 0);
+    if (shape != RS_LONG && ((term | a | y) >> 32) == 0 && rec_short_fits(type, from, flags, n, n1)) {
+        q[0] = make_ulonglong2((u64)rec_short_hdr(type, from, flags, shape, dbit, n, n1) | (term << 32), a | (y << 32));
+        return plane_stored(type, 0);
+    }
+    const u64 H = ((u64)hd & 0x00FFFFFFull) | ((u64)shape << 24) | ((u64)dbit << 31) | (r.w0.y << 32);
     q[0] = make_ulonglong2(H, term); q[RT] = make_ulonglong2(a, y);
-    if (shape != RS_LONG) return false;
+    if (shape != RS_LONG) return plane_stored(type, RF_NOT_SHORT);
     q[2 * RT] = make_ulonglong2(c, d); q[3 * RT] = make_ulonglong2(e, 0);
-    return true;
+    return plane_stored(type, RF_NOT_SHORT | RF_TAIL);
 }
-__device__ __forceinline__ bool rec_has_tail(const ulonglong2& c0) { return ((u32)(c0.x >> 24) & 3u) == RS_LONG; }
 __device__ __forceinline__ Rec rec_decode(const ulonglong2& c0, const ulonglong2& c1, const ulonglong2& t2, const ulonglong2& t3, u32 row)
 {
-    const u64 H = c0.x, term = c0.y;
+    u64 H = c0.x, term = c0.y, x = c1.x, y = c1.y;
+    if (rec_is_short(c0)) {
+        const u32 S = (u32)c0.x;
+        H = (u64)short_hlo(S) | ((u64)short_nn(S) << 32);
+        term = c0.x >> 32; x = c0.y & 0xffffffffull; y = c0.y >> 32;
+    }
     const u32 shape = (u32)(H >> 24) & 3u;
     const u64 dbit = (H >> 31) & 1ull;
     Rec r;
     r.w0.x = (u64)row | ((H & 0x00FFFFFFull) << 32);
     r.w0.y = H >> 32;
-    r.w1.x = term; r.w1.y = c1.x;
-    r.w2.x = shape == RS_AER ? term : c1.y;
-    r.w2.y = shape == RS_LONG ? t2.x : shape == RS_REPLY ? term : shape == RS_AER ? c1.y : 0ull;
+    r.w1.x = term; r.w1.y = x;
+    r.w2.x = shape == RS_AER ? term : y;
+    r.w2.y = shape == RS_LONG ? t2.x : shape == RS_REPLY ? term : shape == RS_AER ? y : 0ull;
     r.w3.x = shape == RS_LONG ? t2.y : shape == RS_REPLY ? dbit : shape == RS_AER ? (dbit ? term : 0ull) : 0ull;
     r.w3.y = shape == RS_LONG ? t3.x : 0ull;
     return r;
@@ -104,8 +154,9 @@ __device__ __forceinline__ bool rec_decode(const ulonglong2& c0, const ulonglong
 __device__ __forceinline__ Rec ld_rec_plane(const ulonglong2* base, u32 tiles, u32 plane, u32 row)
 {
     const ulonglong2* q = base + rec_word(tiles, plane, row, 0);
-    const ulonglong2 c0 = q[0], c1 = q[RT];
-    ulonglong2 t2 = make_ulonglong2(0, 0), t3 = t2;
+    const ulonglong2 c0 = q[0];
+    ulonglong2 c1 = make_ulonglong2(0, 0), t2 = c1, t3 = c1;
+    if (!rec_is_short(c0)) c1 = q[RT];
     if (rec_has_tail(c0)) { t2 = q[2 * RT]; t3 = q[3 * RT]; }
     return rec_decode(c0, c1, t2, t3, row);
 }
@@ -156,8 +207,8 @@ __device__ __forceinline__ void st_rec(ra_event* p, const Rec& r)
     q[0] = make_ulonglong2((u64)r.row | ((u64)r.hdr << 32), (u64)r.nn | ((u64)r.seq << 32));
     q[1] = make_ulonglong2(W(r.term), W(r.a)); q[2] = make_ulonglong2(W(r.b), W(r.c)); q[3] = make_ulonglong2(W(r.d), W(r.e));
 }
-enum { RS_LONG = 0, RS_PLAIN = 1, RS_REPLY = 2, RS_AER = 3 };
-__device__ __forceinline__ bool st_rec_plane(ulonglong2* base, u32 tiles, u32 plane, u32 row, const Rec& r)
+// (every value of a narrow record is below 2^31, so only the header decides whether it is written short)
+__device__ __forceinline__ u32 st_rec_plane(ulonglong2* base, u32 tiles, u32 plane, u32 row, const Rec& r)
 {
     const ix_t term = r.term, a = r.a, b = r.b, c = r.c, d = r.d, e = r.e;
     u32 shape = RS_LONG, dbit = 0;
@@ -167,22 +218,32 @@ __device__ __forceinline__ bool st_rec_plane(ulonglong2* base, u32 tiles, u32 pl
         else if (c == term && d <= 1) { shape = RS_REPLY; dbit = (u32)d; }
         else if (b == term && (d == 0 || d == term)) { shape = RS_AER; y = c; dbit = d != 0; }
     }
-    const u64 H = (u64)((r.hdr & 0x00FFFFFFu) | (shape << 24) | (dbit << 31)) | ((u64)r.nn << 32);
+    const u32 type = r.hdr & 0xffu, from = (r.hdr >> 8) & 0xffu, flags = (r.hdr >> 16) & 0xffu;
     ulonglong2* q = base + rec_word(tiles, plane, row, 0);
+    if (shape != RS_LONG && rec_short_fits(type, from, flags, r.nn & 0xffffu, r.nn >> 16)) {
+        q[0] = make_ulonglong2((u64)rec_short_hdr(type, from, flags, shape, dbit, r.nn & 0xffffu, r.nn >> 16) | (W(term) << 32),
+                               W(a) | (W(y) << 32));
+        return plane_stored(type, 0);
+    }
+    const u64 H = (u64)((r.hdr & 0x00FFFFFFu) | (shape << 24) | (dbit << 31)) | ((u64)r.nn << 32);
     q[0] = make_ulonglong2(H, W(term)); q[RT] = make_ulonglong2(W(a), W(y));
-    if (shape != RS_LONG) return false;
+    if (shape != RS_LONG) return plane_stored(type, RF_NOT_SHORT);
     q[2 * RT] = make_ulonglong2(W(c), W(d)); q[3 * RT] = make_ulonglong2(W(e), 0);
-    return true;
+    return plane_stored(type, RF_NOT_SHORT | RF_TAIL);
 }
-__device__ __forceinline__ bool rec_has_tail(const ulonglong2& c0) { return ((u32)(c0.x >> 24) & 3u) == RS_LONG; }
 // false: some field does not fit the narrow pass (the event stalls to the general kernel, undecoded)
 __device__ __forceinline__ bool rec_decode(const ulonglong2& c0, const ulonglong2& c1, const ulonglong2& t2, const ulonglong2& t3,
                                            u32 row, Rec& r)
 {
-    const u32 Hlo = (u32)c0.x, shape = (Hlo >> 24) & 3u, dbit = Hlo >> 31;
-    const u32 term = (u32)c0.y, x = (u32)c1.x, y = (u32)c1.y;
-    u32 big = (u32)(c0.y >> 32) | (u32)(c1.x >> 32) | (u32)(c1.y >> 32) | ((term | x | y) >> 30);
-    r.row = row; r.hdr = Hlo & 0x00FFFFFFu; r.nn = (u32)(c0.x >> 32); r.seq = 0;
+    u32 Hlo = (u32)c0.x, nn = (u32)(c0.x >> 32), term = (u32)c0.y, x = (u32)c1.x, y = (u32)c1.y;
+    u32 big = (u32)(c0.y >> 32) | (u32)(c1.x >> 32) | (u32)(c1.y >> 32);
+    if (rec_is_short(c0)) {                                     // (chunk 1 is not this record's)
+        Hlo = short_hlo((u32)c0.x); nn = short_nn((u32)c0.x);
+        term = (u32)(c0.x >> 32); x = (u32)c0.y; y = (u32)(c0.y >> 32); big = 0;
+    }
+    big |= (term | x | y) >> 30;
+    const u32 shape = (Hlo >> 24) & 3u, dbit = Hlo >> 31;
+    r.row = row; r.hdr = Hlo & 0x00FFFFFFu; r.nn = nn; r.seq = 0;
     r.term = term; r.a = x;
     if (shape == RS_LONG) {
         big |= (u32)(t2.x >> 32) | (u32)(t2.y >> 32) | (u32)(t3.x >> 32) | (((u32)t2.x | (u32)t2.y | (u32)t3.x) >> 30);
@@ -234,8 +295,9 @@ struct Member {
     // outputs
     u32 n_msgs, n_notes;
     u32 status;                 // RA_ST_* (bits 0-15) | role at the start of the step << 16 | fatal code << 20 | host events not consumed << 28
-    u32 wk;                     // WAL_APPEND notes of this step: count (0..2) | index of the last << 4 | of the one before << 8
-    u32 sent_to;                // 4 bits per peer slot: records put in (me -> slot) this step
+    u32 wk;                     // WAL_APPEND notes of this step: count (0..2) | index of the last << 4 | of the one before << 8,
+                                // and bit 16 + slot: some record put in (me -> slot) this step is not short (count byte bit 4)
+    u32 sent_to;                // 4 bits per peer slot: records put in (me -> slot) this step | some has a tail << 3
     // one note kept back so that a continuing WAL_APPEND / APPLY can merge into it
     u32 pn_type, pn_slot; ix_t pn_a, pn_b, pn_c;
     // flood host model: the last two finalised WAL_APPEND notes
@@ -625,12 +687,19 @@ __device__ __forceinline__ void note_store(Member& m, u32 k, u32 type, u32 slot,
     note_store_raw(&m.C->onote[(size_t)k * m.C->rows + m.row], m.row, type, slot, aux, a, b, c);
 }
 
-// a host ("local") event record into tiled plane k; out of line for the same reason
-__device__ __noinline__ void put_local(ulonglong2* loc, u32 tiles, u32 k, u32 row, u32 type, u32 n, u64 term, u64 a, u64 b)
+// a host ("local") event record (RS_PLAIN) into tiled plane k; out of line for the same reason.
+// Returns RF_NOT_SHORT when it had to be written as a head (loc_n bit 12 + k).
+__device__ __noinline__ u32 put_local(ulonglong2* loc, u32 tiles, u32 k, u32 row, u32 type, u32 flags, u32 n, u64 term, u64 a, u64 b)
 {
-    ulonglong2* q = loc + rec_word(tiles, k, row, 0);               // RS_PLAIN: head only
-    q[0] = make_ulonglong2((u64)type | ((u64)RA_NO_SLOT << 8) | ((u64)RS_PLAIN << 24) | ((u64)(n & 0xffff) << 32), term);
+    ulonglong2* q = loc + rec_word(tiles, k, row, 0);
+    if (((term | a | b) >> 32) == 0 && rec_short_fits(type, RA_NO_SLOT, flags, n, 0)) {
+        q[0] = make_ulonglong2((u64)rec_short_hdr(type, RA_NO_SLOT, flags, RS_PLAIN, 0, n, 0) | (term << 32), a | (b << 32));
+        return plane_stored(type, 0);
+    }
+    q[0] = make_ulonglong2((u64)type | ((u64)RA_NO_SLOT << 8) | ((u64)(flags & 0xff) << 16) | ((u64)RS_PLAIN << 24) |
+                           ((u64)(n & 0xffff) << 32), term);
     q[RT] = make_ulonglong2(a, b);
+    return plane_stored(type, RF_NOT_SHORT);
 }
 
 // `aux`: the row's step flags when this is the last note of the step and no STATUS note follows
@@ -640,7 +709,7 @@ __device__ __forceinline__ void note_flush(Member& m, u32 aux = 0)
     note_store(m, m.n_notes - 1, m.pn_type, m.pn_slot, aux, W(m.pn_a), W(m.pn_b), W(m.pn_c));
     if (m.pn_type == RA_NOTE_WAL_APPEND) {          // the flood host model reads the last two back (row_end_of_step)
         const u32 n = m.wk & 3u;
-        m.wk = (n < 2 ? n + 1 : 2u) | ((m.n_notes - 1) << 4) | ((m.wk & 0xf0u) << 4);
+        m.wk = (m.wk & ~0xfffu) | (n < 2 ? n + 1 : 2u) | ((m.n_notes - 1) << 4) | ((m.wk & 0xf0u) << 4);
     }
     m.pn_type = RA_NOTE_NONE;
 }
@@ -695,7 +764,8 @@ __device__ __forceinline__ void emit_msg(Member& m, u32 to, Rec r)
             const bool peer = MTR == TR_RUNTIME ? (C.peer_mode != 0) : (MTR == TR_PEER);
             if (peer) {
                 // NVLink peer store into the destination GPU's mailbox plane (same local row index)
-                if (st_rec_plane(C.peer_mbox[m.nb][ds], C.tiles, m.slot * RA_MBOX_DEPTH + k, dst, r)) m.sent_to |= 8u << (4 * to);
+                const u32 f = st_rec_plane(C.peer_mbox[m.nb][ds], C.tiles, m.slot * RA_MBOX_DEPTH + k, dst, r);
+                m.sent_to |= (f & RF_TAIL) << (4 * to + 2); m.wk |= (f & RF_NOT_SHORT) << (16 + to);
                 m.sent_to += 1u << (4 * to);
                 m.c_pack += 1u << 8;
                 return;
@@ -716,7 +786,8 @@ __device__ __forceinline__ void emit_msg(Member& m, u32 to, Rec r)
                 return;
             }
         }
-        if (st_rec_plane(C.mbox[m.nb], C.tiles, m.slot * RA_MBOX_DEPTH + k, dst, r)) m.sent_to |= 8u << (4 * to);
+        const u32 f = st_rec_plane(C.mbox[m.nb], C.tiles, m.slot * RA_MBOX_DEPTH + k, dst, r);
+        m.sent_to |= (f & RF_TAIL) << (4 * to + 2); m.wk |= (f & RF_NOT_SHORT) << (16 + to);
         m.sent_to += 1u << (4 * to);
         m.c_pack += 1u << 8;
         return;

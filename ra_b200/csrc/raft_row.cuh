@@ -127,18 +127,19 @@ __device__ __forceinline__ void row_mark_wide(const Cols& C, u32 r, const Member
 // ---- bucket transport: one record another shard sent to a member of this engine ---------------
 // -> mailbox plane of the next step.  The slot is fixed by the record itself (sender slot, k-th
 // record of that sender for this row); byte `from` of the row's count word becomes
-// max(old count, k + 1) | tail flag.
+// max(old count, k + 1) | tail flag (bit 3) | not-short flag (bit 4).
 __device__ __forceinline__ void deliver_record(const Cols& C, const int buf, const Rec& r)
 {
     const u32 row = R_row(r), from = R_from(r), k = (u32)(r.w0.y >> 32);
     if (row >= C.rows || from >= C.members || k >= RA_MBOX_DEPTH) return;
-    const u32 tail = st_rec_plane(C.mbox[buf], C.tiles, from * RA_MBOX_DEPTH + k, row, r) ? 8u : 0u;
+    const u32 f = st_rec_plane(C.mbox[buf], C.tiles, from * RA_MBOX_DEPTH + k, row, r);
+    const u32 size = ((f & RF_TAIL) << 2) | ((f & RF_NOT_SHORT) << 4);
     u32* w = reinterpret_cast<u32*>(&C.mbox_cnt[buf][row]) + (from >> 2);
     const u32 sh = 8u * (from & 3u);
     u32 old = *w;
     for (;;) {
         const u32 ob = (old >> sh) & 0xffu;
-        const u32 nb = ((ob & 7u) >= k + 1 ? (ob & 7u) : k + 1) | (ob & 8u) | tail;
+        const u32 nb = ((ob & 7u) >= k + 1 ? (ob & 7u) : k + 1) | (ob & 0x18u) | size;
         if (nb == ob) break;
         const u32 seen = atomicCAS(w, old, (old & ~(0xffu << sh)) | (nb << sh));
         if (seen == old) break;

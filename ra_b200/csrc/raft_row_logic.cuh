@@ -92,7 +92,7 @@ __device__ __forceinline__ u32 row_end_of_step(Member& m, const Cols& C, u32 r, 
             // (a count byte is zero when its buffer comes round again -- the owner clears the word when it consumes
             // it -- so only senders that sent something have to publish: 1 of a follower's 4 bytes in steady state)
             const u32 nsent = (m.sent_to >> (4 * s)) & 15u;
-            if (nsent) reinterpret_cast<u8*>(&cnt[(size_t)s * C.groups + m.group])[m.slot] = (u8)nsent;
+            if (nsent) reinterpret_cast<u8*>(&cnt[(size_t)s * C.groups + m.group])[m.slot] = (u8)(nsent | (((m.wk >> (16 + s)) & 1u) << 4));
         }
     }
     // record_leader_msg alone (the steady state of a follower) does not get a STATUS note of its own: the
@@ -112,7 +112,7 @@ __device__ __forceinline__ u32 row_end_of_step(Member& m, const Cols& C, u32 r, 
     C.out_n[r] = m.n_msgs | (m.n_notes << 16);
     // flood: synthetic host (DESIGN.md "flood host model")
     if (F.on && !MT_FATAL(m.meta)) {
-        u32 k = 0;
+        u32 k = 0, heads = 0;                               // heads: loc_n bits 12 + k, the records not written short
         bool held = false;                                  // a lagging fsync: this step's notifications are not produced
         if (FAULTS && F.withhold && (m.wk & 3u)) {
             u64 gg0, gr0; flood_ids(C, m, r, gg0, gr0);
@@ -124,15 +124,15 @@ __device__ __forceinline__ u32 row_end_of_step(Member& m, const Cols& C, u32 r, 
         if ((m.wk & 3u) == 2) {
             const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)((m.wk >> 8) & 15u) * C.rows + r]);
             const ulonglong2 h = q[0], t = q[1];
-            put_local(C.loc, C.tiles, k, r, RA_EV_WRITTEN, 0, t.y, h.y, t.x); k++;
+            heads |= put_local(C.loc, C.tiles, k, r, RA_EV_WRITTEN, 0, 0, t.y, h.y, t.x) << (12 + k); k++;
         }
         if ((m.wk & 3u) >= 1) {
             const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)((m.wk >> 4) & 15u) * C.rows + r]);
             const ulonglong2 h = q[0], t = q[1];
-            put_local(C.loc, C.tiles, k, r, RA_EV_WRITTEN, 0, t.y, h.y, t.x); k++;
+            heads |= put_local(C.loc, C.tiles, k, r, RA_EV_WRITTEN, 0, 0, t.y, h.y, t.x) << (12 + k); k++;
         }
         const u32 role = MT_ROLE(m.meta);
-        if (role == RA_LEADER && F.cmds) { put_local(C.loc, C.tiles, k, r, RA_EV_COMMAND, F.cmds, 0, 0, 0); k++; }
+        if (role == RA_LEADER && F.cmds) { heads |= put_local(C.loc, C.tiles, k, r, RA_EV_COMMAND, 0, F.cmds, 0, 0, 0) << (12 + k); k++; }
         u32 idle = MT_IDLE(m.meta);
         if (role == RA_LEADER || (m.status & RA_ST_LEADER_MSG)) idle = 0;
         else if (idle < 15) idle++;
@@ -153,9 +153,9 @@ __device__ __forceinline__ u32 row_end_of_step(Member& m, const Cols& C, u32 r, 
                 if (idle >= 8 + (h2 & 7u)) fire = true;
             }
         }
-        if (fire) { put_local(C.loc, C.tiles, k, r, RA_EV_ELECTION_TIMEOUT, 0, 0, 0, 0); k++; idle = 0; }
+        if (fire) { heads |= put_local(C.loc, C.tiles, k, r, RA_EV_ELECTION_TIMEOUT, 0, 0, 0, 0, 0) << (12 + k); k++; idle = 0; }
         MT_SET(m.meta, 28, 4, idle);
-        C.loc_n[r] = k;
+        C.loc_n[r] = k | heads;
     }
     return fatal;
 }

@@ -56,16 +56,18 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     constexpr u32 NPM = (MMEM ? MMEM : RA_MAX_MEMBERS) * RA_MBOX_DEPTH;
     typedef typename PlaneMask<(NPM + RA_LOCAL_CAP <= 32)>::type mask_t;
     mask_t mine = 0;
-    u32 my_tail = 0;                                            // senders (bits 0..7) / host slots (8..)
-    if (valid && !fatal0) {                                     // whose records carry a 32-byte tail
+    // senders (bits 0..7) / host slots (8..11) whose records carry a 32-byte tail, and the same + 16: whose
+    // records are not all short
+    u32 my_tail = 0;
+    if (valid && !fatal0) {
         u32 mb = 0;
         for (u32 s = 0; s < NMEM(C); s++) {
             const u32 c = (u32)(cntw >> (8 * s)) & 0xffu;
             mb |= ((1u << (c & 7u)) - 1u) << (RA_MBOX_DEPTH * s);
-            my_tail |= ((c >> 3) & 1u) << s;
+            my_tail |= (((c >> 3) & 1u) | (((c >> 4) & 1u) << 16)) << s;
         }
         mine = (mask_t)mb | ((mask_t)((1u << (nloc & 7u)) - 1u) << NPM);
-        my_tail |= nloc & 0xff00u;
+        my_tail |= (nloc & 0x0f00u) | ((nloc & 0xf000u) << 12);
     }
     const bool work = valid && (F.on || nloc || cntw || pending);
     // everything below is per warp: no CTA-wide barrier anywhere in this kernel
@@ -96,7 +98,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     bool stalled = false;
     u32 stall_flags = 0;
 
-    // ---- inputs: TMA stages this warp's record tiles through a ring of NST 2 KB slots, in ------
+    // ---- inputs: TMA stages this warp's record tiles (512 B, 1 KB or 2 KB of each) through a ring of NST 2 KB slots, in
     // evaluation order: deferred pipeline pass, mailbox planes by sender slot then depth, then
     // the host-event planes.  A slot is refilled as soon as the warp has consumed it.
     mask_t rem = 0;                                             // a stalled row's planes not yet evaluated
@@ -117,7 +119,8 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
                 const ulonglong2* src = (q < NPM ? C.mbox[cur] + (size_t)q * plane_words
                                                  : C.loc + (size_t)(q - NPM) * plane_words) + (size_t)wtile * (4 * RT);
                 const u32 tbit = q < NPM ? q / RA_MBOX_DEPTH : 8u + q - NPM;
-                const u32 bytes = ((w_tail >> tbit) & 1u) ? TILE_BYTES : TILE_BYTES / 2;
+                // chunk 0 (512 B) for short records only, 0 + 1 for heads, all four for tails (a tail is not short)
+                const u32 bytes = (TILE_BYTES / 4) << (((w_tail >> tbit) & 1u) + ((w_tail >> (tbit + 16)) & 1u));
                 fence_proxy_async();                            // the slot was read through the generic proxy
                 mbar_expect_tx(&bars[st_issue], bytes);
                 tma_load_tile(&S.stage[warp][st_issue][0], src, bytes, &bars[st_issue]);
@@ -171,7 +174,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
             q[1] = make_ulonglong2((u64)(m.n_msgs | (m.n_notes << 16)) | ((u64)m.status << 32),
                                    (u64)m.sent_to | ((u64)(m.pn_type | (m.pn_slot << 8) | (m.wk << 16)) << 32));
             q[2] = make_ulonglong2(W(m.pn_a), W(m.pn_b));
-            q[3] = make_ulonglong2(W(m.pn_c), 0);
+            q[3] = make_ulonglong2(W(m.pn_c), (u64)(m.wk >> 16));
         }
     }
     flush_counters(C, lane, k_events, k_commits, k_applied, k_msgs, k_dropped, k_elect, k_fatal);
