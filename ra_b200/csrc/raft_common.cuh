@@ -159,8 +159,8 @@ struct StallCtx {                      // 4 x 16 bytes
     u64 pn_a, pn_b;
     u64 pn_c;
     // Member::wk >> 16 -- the per-peer "sent a record that is not short" bits; pn_type_slot_wk keeps its low 16 bits.
-    // (_pad is the name the host emulation knows this word by: it stores 0 there, which is exact for it because its
-    // readers decode every record from the record's own chunk 0 and never use the size flags of the counts.)
+    // A stalled row's end of step publishes them in the count bytes, which size the receiver's fetch in the next step,
+    // so they must survive the stall.  The host emulation carries them the same way (tests/emu: step_row, general_row).
     union { u64 wk_hi; u64 _pad; };
 };
 #define STALL_PENDING 1u               // the deferred pipeline pass has not run yet

@@ -5,7 +5,9 @@
  * head/tail codec, row_end_of_step, load_row / read_row ...) are compiled here as plain C++
  * through tests/emu/cuda_shim.h and driven one row at a time with the control flow of
  * raft_step_kernel (fast paths until a row stalls) and raft_general_kernel (resume from the
- * 64-byte stall context).  What is NOT covered is the kernels' own frame in engine.cu (TMA ring,
+ * 64-byte stall context).  Of the hot kernel's TMA fetch it models what a row can see: how many
+ * chunks of a record tile the size flags let through (the rest reads as poison, see tile_sizes).
+ * What is NOT covered is the rest of the kernels' own frame in engine.cu (the TMA ring itself,
  * warp reductions, launch plumbing): that is what the `-m gpu` tests are for.  The point of this
  * library is that the CPU test tier diffs the very source the GPU runs against the oracle
  * (tests/test_emu_parity.py), so a logic regression shows up before any GPU time is spent.
@@ -166,6 +168,47 @@ struct Scratch { ulonglong2 nm[RA_MAX_MEMBERS]; u64 cs[RA_MAX_MEMBERS]; };   // 
 static unsigned long long g_narrow_stats[3];
 extern "C" void ra_emu_narrow_stats(unsigned long long* out, int reset)
 { for (int i = 0; i < 3; i++) { out[i] = g_narrow_stats[i]; if (reset) g_narrow_stats[i] = 0; } }
+// test observability: stall contexts handed to the general kernel, and those of them whose wk_hi (the per-peer "sent a
+// record that is not short" bits) is not zero
+static unsigned long long g_stall_stats[2];
+extern "C" void ra_emu_stall_stats(unsigned long long* out, int reset)
+{ for (int i = 0; i < 2; i++) { out[i] = g_stall_stats[i]; if (reset) g_stall_stats[i] = 0; } }
+
+// The hot kernel's fetch (raft_step_kernel.cuh): per record tile and plane, TMA stages 512 B (chunk 0), 1 KB (chunks
+// 0-1) or 2 KB (chunks 0-3), as the size flags the warp ORs over its tile say.  The rest of the staging slot holds an
+// earlier tile's bytes.  step_row reads a poison pattern there instead of the record, so a size flag that a writer
+// failed to set shows as a result that differs from the oracle.  The poison decodes to values below 2^30: the narrow
+// pass must take it for a plausible record rather than refuse it to the general path (which reads the plane again).
+// (Which planes a tile fetches, and the ring's depth, do not matter: a row reads only its own planes, and every byte
+// past the fetched length is poison whatever the slot held before.)
+// Whether a poisoned record changes the outcome depends on the record; the count of records the hot path decoded
+// from bytes the kernel would not have fetched does not (ra_emu_fetch_stats: it stays 0 while every flag is right).
+static int g_poison;
+static unsigned long long g_underfetch;
+extern "C" void ra_emu_set_fetch_poison(int pattern) { g_poison = pattern; }
+extern "C" void ra_emu_fetch_stats(unsigned long long* out, int reset) { out[0] = g_underfetch; if (reset) g_underfetch = 0; }
+static ulonglong2 fetch_poison(u32 chunk, u32 row)
+{
+    if (g_poison == 0) return make_ulonglong2(2 * chunk + 1, 2 * chunk + 2);
+    return make_ulonglong2(0x2345678u + 977u * row + chunk, 0x1234567u + 131u * row + 7u * chunk);
+}
+// the warp's size flags (raft_step_kernel.cuh: w_tail): bit s / 16 + s: a record from sender slot s has a tail / is
+// not short; bit 8 + k / 24 + k: the same for host slot k.  Taken at the start of the tile, before any of its rows runs.
+static u32 tile_sizes(const Cols& C, int cur, u32 r0)
+{
+    u32 w = 0;
+    for (u32 r = r0; r < r0 + RT && r < C.rows; r++) {
+        if (MT_FATAL(C.ap[r].y)) continue;
+        const u64 cntw = C.routed ? C.mbox_cnt[cur][r] : 0;
+        const u32 nloc = C.loc_n[r];
+        for (u32 s = 0; s < C.members; s++) {
+            const u32 c = (u32)(cntw >> (8 * s)) & 0xffu;
+            w |= (((c >> 3) & 1u) | (((c >> 4) & 1u) << 16)) << s;
+        }
+        w |= (nloc & 0x0f00u) | ((nloc & 0xf000u) << 12);
+    }
+    return w;
+}
 
 namespace ra_wide {
 #define RA_NARROW_PASS 0
@@ -196,7 +239,7 @@ static void general_row(const Cols& C, int cur, const FloodArgs& F, const StallC
     m.lrs_ok = 0;
     m.n_msgs = ctx.n_msgs_notes & 0xffffu; m.n_notes = (ctx.n_msgs_notes >> 16) & 0xffffu; m.status = ctx.status;
     m.sent_to = ctx.sent_to;
-    { const u32 w = ctx.pn_type_slot_wk; m.pn_type = w & 0xffu; m.pn_slot = (w >> 8) & 0xffu; m.wk = w >> 16; }
+    { const u32 w = ctx.pn_type_slot_wk; m.pn_type = w & 0xffu; m.pn_slot = (w >> 8) & 0xffu; m.wk = (w >> 16) | ((u32)ctx.wk_hi << 16); }
     m.pn_a = ctx.pn_a; m.pn_b = ctx.pn_b; m.pn_c = ctx.pn_c;
     u64 big = 0;
     if (flags & STALL_PENDING) {
@@ -237,19 +280,21 @@ static int run_step(ra_emu* e, const FloodArgs& F)
     }
     // same choice of specialisation as launch_step() in engine.cu
     const int tr = !C.routed ? TR_HOST : (C.n_shards > 1 ? TR_BUCKET : TR_LOCAL);
+    u32 w_tail = 0;
     for (u32 r = 0; r < C.rows; r++) {
+        if ((r & (RT - 1)) == 0) w_tail = tile_sizes(C, e->cur, r);
         StallCtx ctx;
         bool stalled;
         if (C.members == 5) {
             switch (tr) {
             // (narrow pass for the same specialisations as launch_step(); RA_STEP_WIDE=1 keeps the 64-bit pass)
-            case TR_LOCAL:  stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, ctx)
-                                                : ra_wide::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, ctx); break;
-            case TR_BUCKET: stalled = ra_wide::step_row<MK_MM(5, TR_BUCKET)>(C, e->cur, F, r, ctx); break;
-            default:        stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, ctx)
-                                                : ra_wide::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, ctx); break;
+            case TR_LOCAL:  stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, w_tail, ctx)
+                                                : ra_wide::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, w_tail, ctx); break;
+            case TR_BUCKET: stalled = ra_wide::step_row<MK_MM(5, TR_BUCKET)>(C, e->cur, F, r, w_tail, ctx); break;
+            default:        stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, w_tail, ctx)
+                                                : ra_wide::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, w_tail, ctx); break;
             }
-        } else stalled = ra_wide::step_row<MK_MM(0, TR_RUNTIME)>(C, e->cur, F, r, ctx);
+        } else stalled = ra_wide::step_row<MK_MM(0, TR_RUNTIME)>(C, e->cur, F, r, w_tail, ctx);
         // the general kernel runs after the step kernel; rows only ever write to OTHER rows' mailboxes of
         // the NEXT step, so handling a stalled row right away is the same thing
         if (stalled) general_row(C, e->cur, F, ctx);
@@ -324,10 +369,12 @@ extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
         if (len > RA_LOCAL_CAP) { if (err < 2) err = 2; continue; }
         if (C.loc_n[row] != 0) { if (err < 1) err = 1; continue; }
         C.loc_n[row] = len;
-        u32 tails = 0;
-        for (u32 k = 0; k < len; k++)
-            if (st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]))) tails |= 0x100u << k;
-        C.loc_n[row] |= tails;
+        u32 size = 0;                                            // loc_n bits 8 + k (tail), 12 + k (not short)
+        for (u32 k = 0; k < len; k++) {
+            const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]));
+            size |= (((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12)) << k;
+        }
+        C.loc_n[row] |= size;
     }
     if (err) {
         for (u32 r = 0; r < R; r++) C.loc_n[r] = 0;

@@ -59,6 +59,27 @@ class Emu(abi.Backend):
         lib().ra_emu_narrow_stats(arr, 1 if reset else 0)
         return dict(rows_narrow=arr[0], records_refused=arr[1], rows_wide=arr[2])
 
+    @staticmethod
+    def stall_stats(reset: bool = True) -> dict:
+        """Process-wide: stall contexts the hot kernel's logic handed to the general path, and those of them that
+        carried per-peer "not short" bits (StallCtx::wk_hi) across the stall."""
+        arr = (C.c_ulonglong * 2)()
+        lib().ra_emu_stall_stats(arr, 1 if reset else 0)
+        return dict(stalls=arr[0], stalls_wk_hi=arr[1])
+
+    @staticmethod
+    def underfetched(reset: bool = True) -> int:
+        """Process-wide: records the hot kernel's logic decoded although the size flags of their tile did not let the
+        kernel fetch all of their chunks (0 while every writer sets its flags)."""
+        arr = (C.c_ulonglong * 1)()
+        lib().ra_emu_fetch_stats(arr, 1 if reset else 0)
+        return int(arr[0])
+
+    @staticmethod
+    def set_fetch_poison(pattern: int) -> None:
+        """Process-wide: which poison pattern stands for the bytes the hot kernel did not fetch (0 or 1)."""
+        lib().ra_emu_set_fetch_poison(pattern)
+
     def stall_histogram(self) -> dict:
         arr = (C.c_uint64 * 128)()
         self._check(lib().ra_emu_stall_histogram(self._h, arr), "stall_histogram")
