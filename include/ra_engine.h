@@ -294,7 +294,9 @@ enum ra_status {
     RA_E_UNGROUPED = -4,  /* events of one row are not adjacent in the batch */
     RA_E_CAPACITY = -5,   /* more than RA_LOCAL_CAP events for one row, or out buffers too small */
     RA_E_NODEVICE = -6,
-    RA_E_BUSY = -7        /* submit/collect: no free slot, or a submitted batch is still to be collected */
+    RA_E_BUSY = -7,       /* submit/collect: no free slot, or a submitted batch is still to be collected */
+    RA_E_PENDING = -8     /* collect: not evaluated, no row has changed -- the call before it ended in RA_E_CAPACITY for
+                             its outputs; ra_engine_fetch_output them, then submit this batch again */
 };
 
 /* Lifecycle.  The engine owns the HBM Struct-of-Arrays; callers own all host buffers and
@@ -365,8 +367,12 @@ int  ra_engine_step(ra_engine* e,
  * n_ev * CAP is not a bound -- rows * CAP is.  A call whose outputs exceed msgs_cap / notes_cap returns
  * RA_E_CAPACITY with *n_msgs / *n_notes = the sizes needed; the step HAS been evaluated and nothing is lost:
  * the outputs stay in the engine until ra_engine_fetch_output takes them (no other step call is accepted
- * before that).  RA_E_CAPACITY for more than RA_LOCAL_CAP events of one row, RA_E_UNGROUPED and RA_E_INVAL
- * (bad row / type) reject the whole batch: no row has changed.
+ * before that).  ra_engine_pending_output reports the same sizes.  In the compact note format *n_notes counts
+ * notes: the buffer needs *n_notes + 2 * ra_engine_last_ext_count(e) units (set by this RA_E_CAPACITY return).
+ * A call already submitted behind it (split phase, below) is not evaluated: its collect returns RA_E_PENDING and
+ * no row has changed, and ra_engine_fetch_output answers RA_E_BUSY until that call is collected.  Fetch, then
+ * submit that batch again.  RA_E_CAPACITY for more than RA_LOCAL_CAP events of one row, RA_E_UNGROUPED and
+ * RA_E_INVAL (bad row / type) reject the whole batch: no row has changed.
  */
 int  ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes);
 int  ra_engine_fetch_output(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
@@ -475,7 +481,10 @@ int  ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev,
  * (ev, msgs, notes) belong to the engine until it is collected.  With several engines (disjoint sets of
  * groups) one host thread keeps all of them busy: submit to each, then collect each.
  * If a batch is rejected (ungrouped / capacity / bad row), collect returns the error, no row has changed, and
- * every call submitted behind it is rejected with the same status.
+ * every call submitted behind it is rejected with the same status.  If a call's outputs do not fit its buffers,
+ * its collect returns RA_E_CAPACITY (see "Capacity" above: nothing is lost) and every call submitted behind it
+ * returns RA_E_PENDING: not evaluated, no row has changed.  Collect them all, ra_engine_fetch_output the outputs,
+ * then submit those batches again in their order.
  */
 int  ra_engine_submit(ra_engine* e, const ra_event* ev, size_t n_ev,
                       ra_event* msgs, size_t msgs_cap, ra_note* notes, size_t notes_cap);
@@ -512,7 +521,8 @@ typedef struct ra_note16 {
 #define RA_N16_EXT        0x80u
 #define RA_N16_SAME_TERM  0x40u
 int    ra_engine_set_note_format(ra_engine* e, int compact);   /* only while no call is in flight */
-size_t ra_engine_last_ext_count(ra_engine* e);                 /* n_ext of the call collected last */
+size_t ra_engine_last_ext_count(ra_engine* e);                 /* n_ext of the call collected (or fetched) last,
+                                                                  also when it returned RA_E_CAPACITY          */
 /* units + extension area -> ra_note records; last_wal_c = the caller's per-row array (n_rows entries, zeroed at
    reset / load / format switch).  Returns the number of notes written (n_notes), or 0 if cap < n_notes. */
 size_t ra_notes16_expand(const ra_note16* units, size_t n_notes, size_t n_ext, uint64_t* last_wal_c,

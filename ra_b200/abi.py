@@ -67,6 +67,7 @@ FATAL_NOTE_OVERFLOW = 7
 
 RA_OK, RA_E_INVAL, RA_E_NOMEM, RA_E_CUDA, RA_E_UNGROUPED, RA_E_CAPACITY, RA_E_NODEVICE = 0, -1, -2, -3, -4, -5, -6
 RA_E_BUSY = -7
+RA_E_PENDING = -8
 
 
 class RaEvent(C.Structure):

@@ -335,16 +335,21 @@ typedef cub::TransformInputIterator<u64, PackCounts, const u32*> PackedIt;
 // What the host reads when a call completes (pinned, mapped: written by gather_out_kernel itself, so a
 // call needs no device->host copy whose size the host would first have to learn).
 struct OutHdr { u64 n_msgs, n_notes; u32 status, n_ext; };    // status: ingest error 1..3 | 0x100 = outputs do not fit
+// Cols::abort value a gather sets when its outputs do not fit: the calls already submitted behind it change nothing
+// (their ingest and step kernels return at once, their gather reports this value) until the host has taken the
+// outputs (ra_engine_fetch_output), and collect answers RA_E_PENDING for them.  Cleared once no call is in flight.
+#define ABORT_OUT_PENDING 4u
 
 // One warp per tile of 32 rows.  The warp's notes (and records) occupy one contiguous range of the output;
 // a small table in shared memory maps every output position to (lane, k), then the range is written in
 // 16-byte chunks, lane-consecutive: every store instruction of the warp is one contiguous 512-byte burst,
 // which is what makes writing straight into HOST memory (PCIe posted writes) efficient.
 // When the totals do not fit the caller's buffers (or the batch was rejected) nothing is written and the
-// per-row slots are left alone, so that ra_engine_fetch_output can gather again.
+// per-row slots are left alone, so that ra_engine_fetch_output can gather again; a misfit also raises
+// ABORT_OUT_PENDING, so that the calls submitted behind this one do not touch those slots.
 __global__ void __launch_bounds__(128)
 gather_out_kernel(const Cols C, const u64* __restrict__ offs, ulonglong2* __restrict__ msgs, const u64 msgs_cap,
-                  ulonglong2* __restrict__ notes, const u64 notes_cap, OutHdr* hdr, const u32* err)
+                  ulonglong2* __restrict__ notes, const u64 notes_cap, OutHdr* hdr, u32* err)
 {
     __shared__ unsigned short tab[4][32 * (RA_NOTE_CAP > RA_MSG_CAP ? RA_NOTE_CAP : RA_MSG_CAP)];
     const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -355,6 +360,7 @@ gather_out_kernel(const Cols C, const u64* __restrict__ offs, ulonglong2* __rest
     const bool fits = tm <= msgs_cap && tn <= notes_cap;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         hdr->n_msgs = tm; hdr->n_notes = tn; hdr->n_ext = 0; hdr->status = bad | (fits ? 0u : 0x100u);
+        if (!bad && !fits) *err = ABORT_OUT_PENDING;
     }
     if (bad || !fits) return;
     const u32 r = tile * 32 + lane;
@@ -431,7 +437,7 @@ __global__ void note_ext_count_kernel(const Cols C, u32* __restrict__ next)
 __global__ void __launch_bounds__(128)
 gather_out16_kernel(const Cols C, const u64* __restrict__ offs, const u32* __restrict__ xoffs,
                     ulonglong2* __restrict__ msgs, const u64 msgs_cap, ulonglong2* __restrict__ units, const u64 units_cap,
-                    OutHdr* hdr, const u32* err)
+                    OutHdr* hdr, u32* err)
 {
     __shared__ unsigned short tab[4][32 * (RA_NOTE_CAP > RA_MSG_CAP ? RA_NOTE_CAP : RA_MSG_CAP)];
     __shared__ u32 s_mask[4][32], s_xb[4][32];
@@ -444,6 +450,7 @@ gather_out16_kernel(const Cols C, const u64* __restrict__ offs, const u32* __res
     const bool fits = tm <= msgs_cap && tn + 2 * tx <= units_cap;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         hdr->n_msgs = tm; hdr->n_notes = tn; hdr->n_ext = (u32)tx; hdr->status = bad | (fits ? 0u : 0x100u);
+        if (!bad && !fits) *err = ABORT_OUT_PENDING;
     }
     if (bad || !fits) return;
     const u32 r = tile * 32 + lane;
@@ -569,13 +576,14 @@ struct ra_engine {
     // (RA_STEP_WIDE=0), 2 never (RA_STEP_WIDE=1).  A performance choice only; results do not depend on it.
     int narrow, narrow_mode;
     int out_pending;                          // the last collect ended in RA_E_CAPACITY: outputs wait in the row slots
+    size_t pend_msgs, pend_notes;             // ... and their sizes (ra_engine_pending_output)
     size_t pred_msgs, pred_notes, pred_ext;   // outputs of the last collected call (sizes the next DMA is enqueued with)
     int compact;                              // notes leave as 16-byte units (ra_engine_set_note_format)
     u32 *d_next, *d_xoffs; void* d_scan_tmp2; size_t scan_tmp2_bytes;   // compact stream: per-row extension counts + scan
     size_t last_ext;                          // extension entries of the last collected call
     int loc_dirty;                            // the flood host model may have left host events queued
     u64* d_offs; void* d_scan_tmp; size_t scan_tmp_bytes;
-    u32* d_err;                               // [0] sticky ingest error (= Cols::abort), [1] peer barrier timeout
+    u32* d_err;                               // [0] sticky ingest error or ABORT_OUT_PENDING (= Cols::abort), [1] peer barrier timeout
     StallCtx* d_stall; u32* d_stall_cnt;      // d_stall_cnt[2]: alternating per step
     ra_row_state* d_rows; size_t d_rows_cap;
     float last_ms; u32 last_launches;
@@ -615,6 +623,7 @@ extern "C" const char* ra_engine_strerror(int st)
     case RA_E_CAPACITY: return "capacity exceeded (RA_LOCAL_CAP per row, or output buffers too small)";
     case RA_E_NODEVICE: return "no CUDA device: the engine has no CPU fallback";
     case RA_E_BUSY: return "a submitted batch has not been collected yet (or both submit slots are in flight)";
+    case RA_E_PENDING: return "not evaluated: the outputs of the call before it did not fit (fetch them, then submit this batch again)";
     default: return "unknown status";
     }
 }
@@ -1004,8 +1013,9 @@ static int finish_slot(ra_engine* e, IoSlot& q, size_t* n_msgs, size_t* n_notes,
     if (n_notes) *n_notes = (size_t)h.n_notes;
     const u32 bad = h.status & 0xffu;
     if (bad) {
-        // the batch was rejected by ingest: the step kernels of this call (and of any call submitted behind it)
-        // did nothing.  Undo this call's buffer flip; once the last such call is collected, clean up.
+        // the batch was rejected by ingest, or submitted behind a call whose outputs did not fit: the step kernels
+        // of this call (and of any call submitted behind it) did nothing.  Undo this call's buffer flip; once the
+        // last such call is collected, clean up.
         if (was_step) { if (e->C.routed) e->cur ^= 1; e->steps--; }
         if (e->io_head == e->io_tail) {
             CK(cudaStreamSynchronize(e->stream));
@@ -1013,9 +1023,15 @@ static int finish_slot(ra_engine* e, IoSlot& q, size_t* n_msgs, size_t* n_notes,
             CK(cudaMemsetAsync(e->d_err, 0, sizeof(u32), e->stream));
             CK(cudaStreamSynchronize(e->stream));
         }
-        return bad == 1 ? RA_E_UNGROUPED : (bad == 2 ? RA_E_CAPACITY : RA_E_INVAL);
+        return bad == ABORT_OUT_PENDING ? RA_E_PENDING : bad == 1 ? RA_E_UNGROUPED : (bad == 2 ? RA_E_CAPACITY : RA_E_INVAL);
     }
-    if (h.status & 0x100u) { e->out_pending = 1; return RA_E_CAPACITY; }   // nothing lost: ra_engine_fetch_output
+    if (h.status & 0x100u) {                                      // nothing lost: ra_engine_fetch_output
+        e->out_pending = 1; e->pend_msgs = (size_t)h.n_msgs; e->pend_notes = (size_t)h.n_notes;
+        e->last_ext = (size_t)h.n_ext;                            // compact: the units needed are n_notes + 2 * n_ext
+        // the gather raised ABORT_OUT_PENDING; with no call behind this one, lower it now (else that call's collect does)
+        if (e->io_head == e->io_tail) CK(cudaMemsetAsync(e->d_err, 0, sizeof(u32), e->stream));
+        return RA_E_CAPACITY;
+    }
     // top up what the predicted-size copies did not cover (first call, a burst)
     bool more = false;
     if (h.n_msgs > q.copied_msgs) {
@@ -1069,9 +1085,8 @@ extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg*
 extern "C" int ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes)
 {
     if (!e) return RA_E_INVAL;
-    const IoSlot& q = e->io[(e->io_tail + RA_IO_SLOTS - 1) % RA_IO_SLOTS];
-    if (n_msgs) *n_msgs = e->out_pending ? (size_t)q.hdr->n_msgs : 0;
-    if (n_notes) *n_notes = e->out_pending ? (size_t)q.hdr->n_notes : 0;
+    if (n_msgs) *n_msgs = e->out_pending ? e->pend_msgs : 0;
+    if (n_notes) *n_notes = e->out_pending ? e->pend_notes : 0;
     return RA_OK;
 }
 

@@ -256,9 +256,11 @@ static int collect_part(Driver* s, Part* p, size_t* nn)
     int rc = ra_engine_collect(p->e, &nm, nn);
 #ifndef RA_NO_CUDA
     if (rc == RA_E_CAPACITY) {
-        if (*nn + *nn / 8 > p->notes_cap || !p->last_c.empty()) {   // (compact: the extension count is not known here)
+        // 32-byte slots the outputs need (compact: n_notes units + 2 per extension entry, two units to a slot)
+        const size_t need = p->last_c.empty() ? *nn : (*nn + 2 * ra_engine_last_ext_count(p->e) + 1) / 2;
+        if (need + need / 8 > p->notes_cap) {
             ra_engine_free_host(p->notes);
-            p->notes_cap = *nn * 2 + 1024;
+            p->notes_cap = need * 2 + 1024;
             p->notes = (ra_note*)ra_engine_alloc_host(p->notes_cap * sizeof(ra_note));
         }
         if (nm > p->msgs_cap) {

@@ -140,9 +140,25 @@ static ERL_NIF_TERM counters_nif(ErlNifEnv* env, int argc, const ERL_NIF_TERM ar
  * must stay alive until it is collected: they live in a side table keyed by the engine resource, two slots
  * as in the engine.  submit(Ref, EventsBin) / submit_host(Ref, HostEventsBin) -> ok | {error, Code};
  * collect(Ref) -> {MsgsBin, NotesBin} | {error, Code}. */
-typedef struct { ra_engine** owner; ErlNifBinary ev, m, t; unsigned long used; } pend_t;   /* used = submission number */
+typedef struct { ra_engine** owner; ErlNifBinary ev, m, t; unsigned long used; size_t rec; int rc; } pend_t;
+/* used = submission number, rec = event record size, rc = a status collect must return instead of collecting */
 static pend_t PEND[64];
 static unsigned long PEND_SEQ;
+
+static int submit_pend(ra_engine* e, pend_t* p)
+{
+    const size_t n = p->ev.size / p->rec, mc = p->m.size / sizeof(ra_event), nc = p->t.size / sizeof(ra_note);
+    return p->rec == sizeof(ra_event)
+        ? ra_engine_submit(e, (const ra_event*)p->ev.data, n, (ra_event*)p->m.data, mc, (ra_note*)p->t.data, nc)
+        : ra_engine_submit_host(e, (const ra_host_event*)p->ev.data, n, (ra_event*)p->m.data, mc, (ra_note*)p->t.data, nc);
+}
+
+static pend_t* oldest_pend(ra_engine** e)
+{
+    pend_t* p = NULL;
+    for (int i = 0; i < 64; i++) if (PEND[i].used && PEND[i].owner == e && (!p || PEND[i].used < p->used)) p = &PEND[i];
+    return p;
+}
 
 static ERL_NIF_TERM submit_any(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[], size_t rec)
 {
@@ -157,9 +173,8 @@ static ERL_NIF_TERM submit_any(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv
     memcpy(p->ev.data, ev.data, ev.size);
     if (!enif_alloc_binary(mc * sizeof(ra_event), &p->m)) { enif_release_binary(&p->ev); return status_term(env, RA_E_NOMEM); }
     if (!enif_alloc_binary(nc * sizeof(ra_note), &p->t)) { enif_release_binary(&p->ev); enif_release_binary(&p->m); return status_term(env, RA_E_NOMEM); }
-    int rc = rec == sizeof(ra_event)
-        ? ra_engine_submit(*e, (const ra_event*)p->ev.data, n, (ra_event*)p->m.data, mc, (ra_note*)p->t.data, nc)
-        : ra_engine_submit_host(*e, (const ra_host_event*)p->ev.data, n, (ra_event*)p->m.data, mc, (ra_note*)p->t.data, nc);
+    p->rec = rec; p->rc = RA_OK;
+    int rc = submit_pend(*e, p);
     if (rc) { enif_release_binary(&p->ev); enif_release_binary(&p->m); enif_release_binary(&p->t); return status_term(env, rc); }
     p->owner = e; p->used = ++PEND_SEQ;
     return status_term(env, RA_OK);
@@ -173,14 +188,21 @@ static ERL_NIF_TERM collect_nif(ErlNifEnv* env, int argc, const ERL_NIF_TERM arg
 {
     ra_engine** e;
     if (argc != 1 || !enif_get_resource(env, argv[0], ENG, (void**)&e)) return enif_make_badarg(env);
-    pend_t* p = NULL;                                            /* the oldest pending call of this engine */
-    for (int i = 0; i < 64; i++) if (PEND[i].used && PEND[i].owner == e && (!p || PEND[i].used < p->used)) p = &PEND[i];
+    pend_t* p = oldest_pend(e);                                  /* the oldest pending call of this engine */
     if (!p) return status_term(env, RA_E_INVAL);
     size_t nm = 0, nn = 0;
-    int rc = ra_engine_collect(*e, &nm, &nn);
-    enif_release_binary(&p->ev);
+    int rc = p->rc ? p->rc : ra_engine_collect(*e, &nm, &nn);
     p->used = 0;
-    return finish_outputs(env, *e, rc, &p->m, &p->t, nm, nn);
+    enif_release_binary(&p->ev);
+    if (p->rc) { enif_release_binary(&p->m); enif_release_binary(&p->t); return status_term(env, rc); }
+    /* outputs that did not fit: the call submitted behind this one was not evaluated (RA_E_PENDING).  Collect it,
+     * fetch these outputs, then submit it again with its own buffers -- the caller's next collect returns it. */
+    pend_t* q = rc == RA_E_CAPACITY ? oldest_pend(e) : NULL;
+    int qrc = RA_OK;
+    if (q) { size_t x, y; qrc = ra_engine_collect(*e, &x, &y); }
+    ERL_NIF_TERM out = finish_outputs(env, *e, rc, &p->m, &p->t, nm, nn);
+    if (q) q->rc = qrc == RA_E_PENDING ? submit_pend(*e, q) : qrc;
+    return out;
 }
 
 static ErlNifFunc funcs[] = {

@@ -349,6 +349,17 @@ extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, s
     return RA_OK;
 }
 
+// ra_engine_pending_output: the sizes of outputs a call left in the slots (RA_E_CAPACITY), 0 / 0 otherwise
+extern "C" int ra_emu_pending_output(ra_emu* e, size_t* n_msgs, size_t* n_notes)
+{
+    if (!e) return RA_E_INVAL;
+    size_t tm = 0, tn = 0;
+    for (u32 r = 0; e->out_pending && r < e->C.rows; r++) { tm += e->C.out_n[r] & 0xffffu; tn += e->C.out_n[r] >> 16; }
+    if (n_msgs) *n_msgs = tm;
+    if (n_notes) *n_notes = tn;
+    return RA_OK;
+}
+
 extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
                            ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
                            ra_note* notes, size_t notes_cap, size_t* n_notes)

@@ -1,0 +1,488 @@
+"""Differential fuzz of the engine's host call paths: the ways a real caller (INTEGRATION.md, ra_engine_nif.c,
+ra_hostsim) hands batches over and takes outputs back, each against the oracle with ample buffers in the plain
+format.  States and events come from the generator of tests/test_emu_fuzz.py (rich = True) through the rounds of
+tests/test_kernel_fuzz.py: RPC records and notes in order, every row as raw ra_row_state bytes, counters and query
+state are compared.
+
+- host-event batches, each sent three ways: ra_engine_step_host (32-byte records), ra_engine_submit_host_segs split
+  at random row boundaries, ra_engine_step (64-byte records);
+- two calls in flight: batch t+1 drawn from the oracle's state after step t and submitted before t is collected,
+  with pageable and with pinned output buffers, and output sizes that swing from step to step (the predicted-size
+  copy and its top-up);
+- tight output buffers: RA_E_CAPACITY, ra_engine_pending_output and a fetch of exactly the reported size, in the
+  plain and the compact note format, one and two calls deep;
+- the compact note stream, unit for unit against a reference encoder of the rule in include/ra_engine.h, and the
+  decoder (ra_notes16_expand) on every note form the fuzz produces.
+"""
+import ctypes as C
+import random
+import struct
+
+import pytest
+
+import test_emu_fuzz as fz
+import test_kernel_fuzz as kf
+from oracle_lib import Oracle
+from ra_b200 import abi
+from ra_b200.engine import Engine
+from ra_suite import make_backend
+
+HOST_TYPES = {abi.EV_WRITTEN, abi.EV_COMMAND, abi.EV_ELECTION_TIMEOUT, abi.EV_AWAIT_COND_TIMEOUT, abi.EV_PIPELINE_RPCS,
+              abi.EV_TICK, abi.EV_CONSISTENT_QUERY}
+SZ = C.c_size_t
+
+
+def host_event(rng, st, m):
+    """The rich generator, redrawn until it gives a host-origin kind (written, cmd, cmd_long, etmo, ctmo, tick,
+    pipe with EVF_INFO, cq)."""
+    while True:
+        e = fz.random_event(rng, st, m, rich=True)
+        if e.type in HOST_TYPES:
+            return e
+
+
+def _caps(b):
+    return b.n_rows * abi.RA_MSG_CAP, b.n_rows * abi.RA_NOTE_CAP
+
+
+def _abi(b, name, *argtypes):
+    """an entry point by its include/ra_engine.h name (the emulation library exports the split-phase ones too)"""
+    f = getattr(b._lib, "ra_engine_" + name)
+    f.restype = C.c_int
+    f.argtypes = list(argtypes)
+    return f
+
+
+def _segments(rng, evs):
+    """1..256 pieces cut at row boundaries (a row's events never straddle two), some of them empty"""
+    bounds = [0] + [i for i in range(1, len(evs)) if evs[i].row != evs[i - 1].row] + [len(evs)]
+    cuts = sorted(rng.choice(bounds) for _ in range(rng.randint(1, 256) - 1))
+    edges = [0] + cuts + [len(evs)]
+    return [evs[a:b] for a, b in zip(edges, edges[1:])]
+
+
+class _Seg(C.Structure):
+    _fields_ = [("ev", C.c_void_p), ("n", SZ)]
+
+
+def _call(b, path, evs, rng=None, msgs_cap=None, notes_cap=None):
+    """One batch through `path` with ample buffers -> (msgs, notes)."""
+    mc, nc = _caps(b)
+    mc, nc = msgs_cap or mc, notes_cap or nc
+    if path == "step":
+        return b.step(evs, mc, nc)
+    msgs, notes = (abi.RaEvent * mc)(), (abi.RaNote * nc)()
+    nm, nn = SZ(0), SZ(0)
+    if path == "step_host":
+        ev = (abi.RaHostEvent * max(len(evs), 1))(*[abi.RaHostEvent.of(e) for e in evs])
+        st = _abi(b, "step_host", C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.POINTER(SZ), C.c_void_p, SZ,
+                  C.POINTER(SZ))(b._h, ev, len(evs), msgs, mc, C.byref(nm), notes, nc, C.byref(nn))
+    else:
+        parts = _segments(rng, evs)
+        bufs = [(abi.RaHostEvent * max(1, len(p)))(*[abi.RaHostEvent.of(e) for e in p]) for p in parts]
+        segs = (_Seg * len(parts))(*[_Seg(C.addressof(x), len(p)) for x, p in zip(bufs, parts)])
+        st = _abi(b, "submit_host_segs", C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.c_void_p, SZ)(
+            b._h, segs, len(parts), msgs, mc, notes, nc)
+        assert st == abi.RA_OK
+        st = _abi(b, "collect", C.c_void_p, C.POINTER(SZ), C.POINTER(SZ))(b._h, C.byref(nm), C.byref(nn))
+    assert st == abi.RA_OK, "%s: status %d" % (path, st)
+    return list(msgs[: nm.value]), list(notes[: nn.value])
+
+
+def _checker(o, m, bs, rnd, mode):
+    def check(what, outs, evs):
+        want = kf._observe(o, m, out=outs[0])
+        for (w, p, b), out in zip(bs, outs[1:]):
+            kf._compare(want, kf._observe(b, m, out=out), "M=%d %s round %d RA_STEP_WIDE=%s %s: %s"
+                        % (m, mode, rnd, w, p, what), evs, o)
+    return check
+
+
+# ---- 1. host-event batches, three ways ------------------------------------------------------------------------------
+PATHS = ["step_host", "segs", "step"]
+HOST_MODES = ["routed", "flood"]
+
+
+def _host_fuzz(backend, mode, m, G, rounds, seed, monkeypatch):
+    rng, srng = random.Random(seed), random.Random(seed + 1)
+    o = Oracle(G, m, **kf._kw(mode))
+    bs = []
+    for w in kf.WIDTHS:
+        monkeypatch.setenv("RA_STEP_WIDE", w)
+        bs += [(w, p, make_backend(backend, G, m, **kf._kw(mode))) for p in PATHS]
+    n_long = 0
+    for rnd in range(rounds):
+        loads, qs, events = kf._fuzz_round(rng, o, m, G, rnd, draw=host_event)
+        assert all(e.type in HOST_TYPES for e in events)
+        n_long += sum(1 for e in events if e.type == abi.EV_COMMAND and e.n >= 256)
+        for x in [o] + [b for *_, b in bs]:
+            x.load_rows(loads)
+            x.load_query_state(qs)
+        check = _checker(o, m, bs, rnd, mode)
+
+        def step_all(evs):
+            return [o.step([fz._copy(e) for e in evs])] + [_call(b, p, [fz._copy(e) for e in evs], srng)
+                                                          for _, p, b in bs]
+        for k, evs in enumerate([events] + ([[], []] if mode == "routed" else [])):
+            check("step %d" % k, step_all(evs), evs)
+        if mode == "flood":
+            faults = kf.FAULTS if rnd % 2 else None
+            o.flood(4, kf.FLOOD_CMDS, kf.PERMILLE, seed=seed + rnd, threads=4, faults=faults)
+            for *_, b in bs:
+                b.flood(4, kf.FLOOD_CMDS, kf.PERMILLE, seed=seed + rnd, faults=faults)
+            check("the step after the flood", step_all([]), [])
+    assert n_long > 0                                            # commands of 256 and 1000 entries: n above 8 bits
+    return o
+
+
+@pytest.mark.parametrize("mode", HOST_MODES)
+@pytest.mark.parametrize("m", kf.MEMBERS)
+def test_host_batches_three_ways_emu(m, mode, monkeypatch):
+    _host_fuzz("emu", mode, m, 48, 4, 8000 + 10 * m + HOST_MODES.index(mode), monkeypatch)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", HOST_MODES)
+@pytest.mark.parametrize("m", kf.MEMBERS)
+def test_host_batches_three_ways_engine(m, mode, monkeypatch):
+    _host_fuzz("engine", mode, m, 1200 if m <= 5 else 1024, 2, 8500 + 10 * m + HOST_MODES.index(mode), monkeypatch)
+
+
+# ---- compact note stream: the reference encoder (include/ra_engine.h, "Compact note stream") ------------------------
+def encode16(notes, wal_c):
+    """notes (ordered by row, seq) -> (the bytes of units + extension area, n_ext).  wal_c: row -> c of the row's
+    previous WAL_APPEND note (absent = 0), updated by every WAL_APPEND."""
+    units, ext = [], []
+    for n in notes:
+        small = n.slot == 0 and n.a <= n.b and n.b - n.a < 256
+        if n.type == abi.NOTE_WAL_APPEND:
+            same = n.c == wal_c.get(n.row, 0)
+            wal_c[n.row] = n.c
+            one = small and same
+        else:
+            one = small and n.c == 0
+        if one:
+            t = n.type | (abi.N16_SAME_TERM if n.type == abi.NOTE_WAL_APPEND else 0)
+            units.append(struct.pack("<IBBHQ", n.row, t, n.b - n.a, n.aux, n.a))
+        else:
+            units.append(struct.pack("<IBBHQ", n.row, n.type | abi.N16_EXT, n.slot, n.aux, len(ext) // 2))
+            ext += [struct.pack("<QQ", n.a, n.b), struct.pack("<QQ", n.c, 0)]
+    return b"".join(units + ext), len(ext) // 2
+
+
+def _expand(units, n_notes, n_ext, last_c):
+    from ra_b200.engine import lib
+    f = lib().ra_notes16_expand
+    f.restype = SZ
+    f.argtypes = [C.c_void_p, SZ, SZ, C.c_void_p, C.c_void_p, SZ]
+    out = (abi.RaNote * max(n_notes, 1))()
+    buf = C.create_string_buffer(bytes(units), max(len(units), 1))
+    assert f(buf, n_notes, n_ext, last_c, out, max(n_notes, 1)) == n_notes
+    return list(out[:n_notes])
+
+
+FORMS = ("ext_slot", "range_256", "status_c", "above_2_32", "truncate", "query", "same_term")
+
+
+def _forms(notes, seen):
+    for n in notes:
+        seen["ext_slot"] += n.slot != 0
+        seen["range_256"] += n.b >= n.a + 256
+        seen["status_c"] += n.type == abi.NOTE_STATUS and n.c != 0
+        seen["above_2_32"] += max(n.a, n.b, n.c) >= 1 << 32
+        seen["truncate"] += n.type == abi.NOTE_TRUNCATE
+        seen["query"] += n.type in (abi.NOTE_QUERY_INDEX, abi.NOTE_QUERY_AGREED)
+
+
+class _RoundTrip(Oracle):
+    """CPU tier: the oracle whose notes go through the reference encoder and ra_notes16_expand on their way out."""
+
+    def __init__(self, G, m, **kw):
+        super().__init__(G, m, **kw)
+        self.wal_c, self.last_c = {}, (C.c_uint64 * (G * m))()
+        self.seen = dict.fromkeys(FORMS, 0)
+
+    def load_rows(self, rows):
+        super().load_rows(rows)
+        for s in rows:
+            self.wal_c.pop(s.row, None)
+            self.last_c[s.row] = 0
+
+    def step(self, events, msgs_cap=None, notes_cap=None):
+        msgs, notes = super().step(events, msgs_cap, notes_cap)
+        _forms(notes, self.seen)
+        units, n_ext = encode16(notes, self.wal_c)
+        self.seen["same_term"] += sum(1 for k in range(len(notes)) if units[16 * k + 4] & abi.N16_SAME_TERM)
+        return msgs, _expand(units, len(notes), n_ext, self.last_c)
+
+
+@pytest.mark.parametrize("mode", kf.MODES)
+def test_notes16_expand_on_fuzz_notes(mode):
+    """every note the fuzz produces, through the reference encoder and the host decoder, comes back unchanged"""
+    seen = dict.fromkeys(FORMS, 0)
+    for m in (3, 5, 8):
+        _, bs, _ = kf._fuzz(lambda w, G, m, **kw: _RoundTrip(G, m, **kw), mode, m, 48, 4, 9000 + 10 * m)
+        for _, b in bs:
+            for k, v in b.seen.items():
+                seen[k] += v
+    missing = [k for k in FORMS if not seen[k] and not (k == "query" and mode == "flood")]
+    assert not missing, (missing, seen)
+
+
+class _CompactEngine(Engine):
+    """GPU tier: an Engine in the compact note format whose step() returns the notes ra_notes16_expand rebuilt, after
+    checking its raw units and extension area against the reference encoder on those notes.  Since the fuzz compares
+    the notes with the oracle's, the units equal the encoder's output on the oracle's notes."""
+
+    def __init__(self, G, m, **kw):
+        super().__init__(G, m, **kw)
+        self.set_note_format(True)
+        self.wal_c, self.ext = {}, 0
+
+    def load_rows(self, rows):
+        super().load_rows(rows)
+        for s in rows:                                           # the engine and the decoder forget the row's c
+            self.wal_c.pop(s.row, None)
+            self._last_c[s.row] = 0
+
+    def step(self, events, msgs_cap=None, notes_cap=None):
+        msgs, notes, units, n_ext = self.step_compact(events, msgs_cap=self.n_rows * abi.RA_MSG_CAP)
+        want, want_ext = encode16(notes, self.wal_c)
+        got = b"".join(bytes(u) for u in units)
+        assert (got, n_ext) == (want, want_ext), "compact units differ from the reference encoder"
+        self.ext += n_ext
+        return msgs, notes
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", kf.MODES)
+def test_compact_stream_unit_for_unit_engine(mode, monkeypatch):
+    def make(w, G, m, **kw):
+        monkeypatch.setenv("RA_STEP_WIDE", w)
+        return _CompactEngine(G, m, **kw)
+    _, bs, _ = kf._fuzz(make, mode, 5, 1200, 3, 9500 + kf.MODES.index(mode))
+    assert all(b.ext > 0 for _, b in bs)
+
+
+# ---- raw calls with counts on RA_E_CAPACITY -------------------------------------------------------------------------
+def _pending(b):
+    f = b._fn("pending_output")
+    f.restype = C.c_int
+    f.argtypes = [C.c_void_p, C.POINTER(SZ), C.POINTER(SZ)]
+    nm, nn = SZ(0), SZ(0)
+    assert f(b._h, C.byref(nm), C.byref(nn)) == abi.RA_OK
+    return nm.value, nn.value
+
+
+def _last_ext(b):
+    f = b._lib.ra_engine_last_ext_count
+    f.restype = SZ
+    f.argtypes = [C.c_void_p]
+    return f(b._h)
+
+
+class _Out:
+    """output buffers of one call: pageable ctypes arrays or pinned ra_engine_alloc_host memory; notes_cap counts
+    32-byte notes or (compact) 16-byte units"""
+
+    def __init__(self, b, msgs_cap, notes_cap, compact=False, pinned=False):
+        self.b, self.mc, self.nc, self.compact, self.pinned = b, msgs_cap, notes_cap, compact, pinned
+        nt = abi.RaNote16 if compact else abi.RaNote
+        if pinned:
+            l = b._lib
+            l.ra_engine_alloc_host.restype = C.c_void_p
+            l.ra_engine_alloc_host.argtypes = [SZ]
+            self._p = [l.ra_engine_alloc_host(max(msgs_cap, 1) * 64), l.ra_engine_alloc_host(max(notes_cap, 1) * 32)]
+            assert all(self._p)
+            self.msgs = (abi.RaEvent * max(msgs_cap, 1)).from_address(self._p[0])
+            self.notes = (nt * max(notes_cap, 1)).from_address(self._p[1])
+        else:
+            self.msgs, self.notes = (abi.RaEvent * max(msgs_cap, 1))(), (nt * max(notes_cap, 1))()
+
+    def free(self):
+        if self.pinned:
+            f = self.b._lib.ra_engine_free_host
+            f.restype, f.argtypes = None, [C.c_void_p]
+            for p in self._p:
+                f(p)
+            self.pinned = False
+
+    def result(self, nm, nn, n_ext=0, last_c=None):
+        msgs = [fz._copy(x) for x in self.msgs[:nm]]
+        if not self.compact:
+            return msgs, [abi.RaNote.from_buffer_copy(x) for x in self.notes[:nn]]
+        return msgs, _expand(bytes(self.notes)[: 16 * (nn + 2 * n_ext)], nn, n_ext, last_c)
+
+    def units(self, nn, n_ext):
+        return bytes(self.notes)[: 16 * (nn + 2 * n_ext)]
+
+
+def _submit(b, api, evs, out):
+    if api == "submit_host":
+        ev = (abi.RaHostEvent * max(len(evs), 1))(*[abi.RaHostEvent.of(e) for e in evs])
+    else:
+        ev = (abi.RaEvent * max(len(evs), 1))(*evs)
+    st = _abi(b, api, C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.c_void_p, SZ)(
+        b._h, ev, len(evs), out.msgs, out.mc, out.notes, out.nc)
+    assert st == abi.RA_OK, "%s: status %d" % (api, st)
+    return ev                                                    # (kept alive until collected)
+
+
+def _collect(b):
+    nm, nn = SZ(0), SZ(0)
+    st = _abi(b, "collect", C.c_void_p, C.POINTER(SZ), C.POINTER(SZ))(b._h, C.byref(nm), C.byref(nn))
+    return st, nm.value, nn.value
+
+
+def _fetch(b, out):
+    nm, nn = SZ(0), SZ(0)
+    f = b._fn("fetch_output")
+    f.restype = C.c_int
+    f.argtypes = [C.c_void_p, C.c_void_p, SZ, C.POINTER(SZ), C.c_void_p, SZ, C.POINTER(SZ)]
+    st = f(b._h, out.msgs, out.mc, C.byref(nm), out.notes, out.nc, C.byref(nn))
+    return st, nm.value, nn.value
+
+
+def _batch(rng, o, m, G, draw, density):
+    """a batch drawn from the oracle's current state (no reload: calls may be in flight)"""
+    evs = []
+    for st in o.read_rows(range(G * m)):
+        if rng.random() < density:
+            evs += [draw(rng, st, m) for _ in range(rng.randint(1, abi.RA_LOCAL_CAP))]
+    return evs
+
+
+def _rich(rng, st, m):
+    return fz.random_event(rng, st, m, rich=True)
+
+
+# ---- 2 + 3. two calls in flight; tight output buffers, one and two calls deep ---------------------------------------
+def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compact=False, pinned=False):
+    """rounds of `steps` batches; every batch goes in while `depth - 1` calls are still in flight.  tight: each call's
+    buffers hold 0 .. all of what it needs; a call answered RA_E_CAPACITY is fetched with exactly the reported size,
+    and a call submitted behind it must come back RA_E_PENDING and is submitted again."""
+    draw = host_event if api == "submit_host" else _rich
+    wal_c, last_c = {}, ((C.c_uint64 * (G * m))() if compact else None)
+    cov = dict(capacity=0, pending=0, calls=0)
+    for rnd in range(rounds):
+        loads, qs, _ = kf._fuzz_round(rng, o, m, G, rnd, draw=draw)
+        for x in (o, b):
+            x.load_rows(loads)
+            x.load_query_state(qs)
+        for s in loads:
+            wal_c.pop(s.row, None)
+            if compact:
+                last_c[s.row] = 0
+        wants, fly = [], []                                      # oracle outputs of every batch; calls in flight
+
+        def new_out(k):
+            msgs, notes = wants[k][1]
+            n_units = len(notes)
+            if compact:
+                wants[k][2], wants[k][3] = encode16(notes, dict(wal_c_at[k]))
+                n_units += 2 * wants[k][3]
+            if tight:
+                return _Out(b, rng.randint(0, len(msgs)), rng.randint(0, n_units), compact, pinned)
+            return _Out(b, G * m * abi.RA_MSG_CAP, G * m * abi.RA_NOTE_CAP * (2 if compact else 1), compact, pinned)
+
+        wal_c_at = []
+
+        def submit(k):
+            out = new_out(k)
+            fly.append((k, out, _submit(b, api, wants[k][0], out)))
+
+        def finish(k, out, nm, nn):
+            msgs, notes = wants[k][1]
+            what = "M=%d %s round %d batch %d" % (m, mode, rnd, k)
+            n_ext = 0
+            if compact:
+                n_ext = _last_ext(b)
+                assert n_ext == wants[k][3], "%s: ra_engine_last_ext_count %d, the encoder %d" % (what, n_ext, wants[k][3])
+                assert out.units(nn, n_ext) == wants[k][2], "%s: compact units differ" % what
+            got = out.result(nm, nn, n_ext, last_c)
+            outputs = lambda ms, ns: dict(msgs=[x.key() for x in ms], notes=[x.key() for x in ns], rows=b"",
+                                          counters=0, query=0)
+            kf._compare(outputs(msgs, notes), outputs(*got), what, wants[k][0], o)
+            out.free()
+
+        def collect_oldest():
+            k, out, _ev = fly.pop(0)
+            st, nm, nn = _collect(b)
+            cov["calls"] += 1
+            msgs, notes = wants[k][1]
+            what = "M=%d %s round %d batch %d" % (m, mode, rnd, k)
+            if st == abi.RA_E_CAPACITY:
+                cov["capacity"] += 1
+                assert (nm, nn) == (len(msgs), len(notes)), "%s: RA_E_CAPACITY reports %r, needed %r" % (
+                    what, (nm, nn), (len(msgs), len(notes)))
+                assert _pending(b) == (len(msgs), len(notes)), "%s: pending_output %r" % (what, _pending(b))
+                behind = []
+                while fly:                                       # calls submitted behind it: not evaluated
+                    k2, out2, _ = fly.pop(0)
+                    st2, _, _ = _collect(b)
+                    assert st2 == abi.RA_E_PENDING, "%s: the call submitted behind it returned %d, not " \
+                        "RA_E_PENDING" % (what, st2)
+                    cov["pending"] += 1
+                    out2.free()
+                    behind.append(k2)
+                units = nn + 2 * _last_ext(b) if compact else nn
+                out.free()
+                out = _Out(b, nm, units, compact, pinned)
+                st, nm2, nn2 = _fetch(b, out)
+                assert st == abi.RA_OK and (nm2, nn2) == (nm, nn), "%s: fetch of the reported size: %d %r" % (
+                    what, st, (nm2, nn2))
+                finish(k, out, nm, nn)
+                for k2 in behind:
+                    submit(k2)
+            else:
+                assert st == abi.RA_OK, "%s: collect status %d" % (what, st)
+                finish(k, out, nm, nn)
+
+        for t in range(steps):
+            evs = _batch(rng, o, m, G, draw, rng.choice([0.02, 0.3, 1.0]))
+            wal_c_at.append(dict(wal_c))
+            want = o.step([fz._copy(e) for e in evs], G * m * abi.RA_MSG_CAP, G * m * abi.RA_NOTE_CAP)
+            encode16(want[1], wal_c)                             # the per-row memory the engine keeps
+            wants.append([evs, want, None, 0])
+            submit(t)
+            while len(fly) >= depth:
+                collect_oldest()
+        while fly:
+            collect_oldest()
+        assert kf._rows_bytes(b) == kf._rows_bytes(o), "M=%d %s round %d: rows differ" % (m, mode, rnd)
+        assert b.counters() == o.counters()
+    return cov
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("pinned", [False, True], ids=["pageable", "pinned"])
+@pytest.mark.parametrize("api", ["submit", "submit_host"])
+def test_two_calls_in_flight_engine(api, pinned):
+    G, m = 1200, 5
+    rng = random.Random(9700 + 2 * (api == "submit_host") + pinned)
+    o, b = Oracle(G, m, **kf._kw("chased")), Engine(G, m, **kf._kw("chased"))
+    cov = _chain(b, o, m, G, "chased", api, rng, rounds=2, steps=8, depth=2, pinned=pinned)
+    assert cov["calls"] == 16
+
+
+TIGHT = [("emu", "plain", 1), pytest.param("engine", "plain", 1, marks=pytest.mark.gpu),
+         pytest.param("engine", "compact", 1, marks=pytest.mark.gpu),
+         pytest.param("engine", "plain", 2, marks=pytest.mark.gpu),
+         pytest.param("engine", "compact", 2, marks=pytest.mark.gpu)]
+
+
+@pytest.mark.parametrize("backend,fmt,depth", TIGHT)
+@pytest.mark.parametrize("mode", ["chased", "routed"])
+def test_tight_output_buffers(backend, fmt, depth, mode):
+    """every call gets 0 .. all of the buffer space it needs; what RA_E_CAPACITY reports must be exactly what a
+    fetch needs, and a call in flight behind it must change nothing"""
+    G, m = (48, 5) if backend == "emu" else (1200, 5)
+    rng = random.Random(9800 + 10 * depth + (fmt == "compact") + 100 * (mode == "routed"))
+    o, b = Oracle(G, m, **kf._kw(mode)), make_backend(backend, G, m, **kf._kw(mode))
+    if fmt == "compact":
+        b.set_note_format(True)
+    api = "submit" if backend == "engine" else "submit_host"      # (the emulation has the host-event pair only)
+    cov = _chain(b, o, m, G, mode, api, rng, rounds=2, steps=6, depth=depth, tight=True, compact=fmt == "compact")
+    assert cov["capacity"] > 0
+    if depth == 2:
+        assert cov["pending"] > 0

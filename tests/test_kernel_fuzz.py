@@ -35,8 +35,13 @@ FLOOD_CMDS, PERMILLE = 300, 15
 RELOAD, WIDE_ROWS = 0.7, 0.05               # per round and row: fresh state / moved to the narrow limit
 
 
-def _kw(mode):
-    return dict(pure=(mode == "pure"), route_on_device=mode in ("routed", "flood"), max_aer_batch=512)
+# small note budgets (cfg.note_cap, RA_NOTE_RESERVE + 2 ..) per M, in the order of MODES: every budget meets several
+# modes; the larger ones go where more peers make more notes, so that each case still runs into its budget
+NOTE_CAPS = {3: [6, 7, 6, 7], 4: [7, 6, 7, 6], 5: [9, 6, 9, 7], 7: [12, 6, 7, 9], 8: [9, 12, 6, 9]}
+
+
+def _kw(mode, note_cap=0):
+    return dict(pure=(mode == "pure"), route_on_device=mode in ("routed", "flood"), max_aer_batch=512, note_cap=note_cap)
 
 
 def _observe(b, m, out=None):
@@ -68,8 +73,9 @@ def _compare(want, got, what, events, oracle):
             raise AssertionError("%s: %s differ: oracle %r, got %r" % (what, k, want[k], got[k]))
 
 
-def _fuzz_round(rng, o, m, G, rnd):
-    """States to load and the event batch of one round (events drawn from the oracle's state of rows not reloaded)."""
+def _fuzz_round(rng, o, m, G, rnd, draw=None):
+    """States to load and the event batch of one round (events drawn from the oracle's state of rows not reloaded).
+    draw(rng, state, m) -> event replaces the rich generator (tests/test_call_paths_fuzz.py: host events only)."""
     n_rows = G * m
     cur = o.read_rows(range(n_rows))
     loads, events, qs = [], [], []
@@ -87,20 +93,47 @@ def _fuzz_round(rng, o, m, G, rnd):
                 q.peer_query_index[p] = rng.randint(0, 4)
             qs.append(q)
         for _ in range(rng.randint(0, abi.RA_LOCAL_CAP)):
-            e = fz.random_event(rng, st, m, rich=True)
+            e = draw(rng, st, m) if draw else fz.random_event(rng, st, m, rich=True)
             if shift:
                 fz._shift_event(e, shift[0], shift[1])
             events.append(e)
     return loads, qs, events
 
 
-def _fuzz(make, mode, m, G, rounds, seed):
-    """make(width) -> a backend built with RA_STEP_WIDE = width; returns the backends for the coverage checks."""
+def _unconsumed(notes, events):
+    """The host events a note budget left unconsumed (include/ra_engine.h RA_ST_NOTE_OVERFLOW): STATUS.c bits 8..15 =
+    how many of the LAST events of the row's run in the batch; the caller submits them again."""
+    left = []
+    for n in notes:
+        k = (n.c >> 8) & 0xff if n.type == abi.NOTE_STATUS and n.aux & abi.ST_NOTE_OVERFLOW else 0
+        if k:
+            left += [e for e in events if e.row == n.row][-k:]
+    return left
+
+
+def _snapshot_bursts(rng, loads, m):
+    """Half the loaded leaders with a snapshot need it sent to every peer: their next pipeline pass or tick emits one
+    SEND_SNAPSHOT per peer, a burst of notes that a small budget cannot hold (RA_FATAL_NOTE_OVERFLOW)."""
+    for st in loads:
+        if st.role == abi.LEADER and st.has_snapshot and rng.random() < 0.5:
+            for p in range(m):
+                pe = st.peers[p]
+                pe.next_index = max(1, st.snapshot_index)
+                pe.match_index = min(pe.match_index, pe.next_index - 1)
+
+
+def _fuzz(make, mode, m, G, rounds, seed, note_cap=0):
+    """make(width) -> a backend built with RA_STEP_WIDE = width; returns the oracle, the backends for the coverage
+    checks and what the note budget did.  note_cap != 0: every backend runs with that budget, and after each step the
+    host events it left unconsumed are submitted again in a step of their own (or in the empty step that follows)."""
     rng = random.Random(seed)
-    o = Oracle(G, m, **_kw(mode))
-    bs = [(w, make(w, G, m, **_kw(mode))) for w in WIDTHS]
+    o = Oracle(G, m, **_kw(mode, note_cap))
+    bs = [(w, make(w, G, m, **_kw(mode, note_cap))) for w in WIDTHS]
+    cov = dict(refused=0, fatal_overflow=0)
     for rnd in range(rounds):
         loads, qs, events = _fuzz_round(rng, o, m, G, rnd)
+        if note_cap:
+            _snapshot_bursts(rng, loads, m)
         steps = [events] + ([[], []] if mode == "routed" else [])
         for x in [o] + [b for _, b in bs]:
             x.load_rows(loads)
@@ -112,9 +145,21 @@ def _fuzz(make, mode, m, G, rounds, seed):
                 _compare(want, _observe(b, m, out=out), "M=%d %s round %d RA_STEP_WIDE=%s: %s" % (m, mode, rnd, w, what),
                          evs, o)
 
-        for k, evs in enumerate(steps):
+        k = 0
+        while k < len(steps):
+            evs = steps[k]
             outs = [x.step([fz._copy(e) for e in evs]) for x in [o] + [b for _, b in bs]]
             check("step %d" % k, outs, evs)
+            left = _unconsumed(outs[0][1], evs)
+            cov["refused"] += len(left)
+            cov["fatal_overflow"] += sum(1 for n in outs[0][1] if n.type == abi.NOTE_STATUS and n.aux & abi.ST_FATAL
+                                         and n.c & 0xff == abi.FATAL_NOTE_OVERFLOW)
+            if left:
+                if k + 1 < len(steps):
+                    steps[k + 1] = left + steps[k + 1]
+                else:
+                    steps.append(left)
+            k += 1
         if mode == "flood":
             faults = FAULTS if rnd % 2 else None
             o.flood(4, FLOOD_CMDS, PERMILLE, seed=seed + rnd, threads=4, faults=faults)
@@ -123,7 +168,7 @@ def _fuzz(make, mode, m, G, rounds, seed):
             check("flood%s" % (" with faults" if faults else ""), [([], [])] * (1 + len(bs)), [])
             outs = [x.step([]) for x in [o] + [b for _, b in bs]]
             check("the step after the flood", outs, [])
-    return o, bs
+    return o, bs, cov
 
 
 def _maker(name, monkeypatch):
@@ -138,7 +183,7 @@ def _maker(name, monkeypatch):
 @pytest.mark.parametrize("m", MEMBERS)
 def test_kernel_fuzz_emu(m, mode, monkeypatch):
     Emu.narrow_stats(); Emu.stall_stats(); Emu.underfetched()
-    o, bs = _fuzz(_maker("emu", monkeypatch), mode, m, 64, 12, 4000 + 10 * m + MODES.index(mode))
+    o, bs, _ = _fuzz(_maker("emu", monkeypatch), mode, m, 64, 12, 4000 + 10 * m + MODES.index(mode))
     assert Emu.underfetched() == 0, "the hot path decoded a record from bytes its tile's fetch did not cover"
     assert Emu.stall_stats()["stalls"] > 0
     assert o.counters()["fatal_rows"] > 0
@@ -177,9 +222,38 @@ def test_kernel_fuzz_routed_twin():
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("m", MEMBERS)
 def test_kernel_fuzz_engine(m, mode, monkeypatch):
-    o, bs = _fuzz(_maker("engine", monkeypatch), mode, m, 1200 if m <= 5 else 1024, 3, 7000 + 10 * m + MODES.index(mode))
+    o, bs, _ = _fuzz(_maker("engine", monkeypatch), mode, m, 1200 if m <= 5 else 1024, 3, 7000 + 10 * m + MODES.index(mode))
     for w, b in bs:
         assert b.stall_histogram(), "RA_STEP_WIDE=%s: no row took the general kernel" % w
+
+
+# ---- small note budgets: events refused and submitted again, rows stopped by a burst of notes -----------------------
+def _note_cap_of(m, mode):
+    return NOTE_CAPS[m][MODES.index(mode)]
+
+
+def _budget_coverage(o, m, mode, cov):
+    assert cov["refused"] > 0, "no host event was left unconsumed by the budget"
+    if m >= 7 and mode != "flood":                  # a burst of 6-7 SEND_SNAPSHOT notes (the flood case has one
+        assert cov["fatal_overflow"] > 0, "no row stopped with RA_FATAL_NOTE_OVERFLOW"       # fuzzed step only)
+    if mode in ("routed", "flood"):
+        assert o.counters()["msgs_dropped"] > 0
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("m", MEMBERS)
+def test_kernel_fuzz_note_cap_emu(m, mode, monkeypatch):
+    o, _, cov = _fuzz(_maker("emu", monkeypatch), mode, m, 64, 8, 4500 + 10 * m + MODES.index(mode), _note_cap_of(m, mode))
+    _budget_coverage(o, m, mode, cov)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("m", [3, 5, 8])
+def test_kernel_fuzz_note_cap_engine(m, mode, monkeypatch):
+    o, _, cov = _fuzz(_maker("engine", monkeypatch), mode, m, 1024, 2, 7500 + 10 * m + MODES.index(mode),
+                      _note_cap_of(m, mode))
+    _budget_coverage(o, m, mode, cov)
 
 
 @pytest.mark.gpu
