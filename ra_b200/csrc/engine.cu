@@ -145,6 +145,29 @@ __device__ __forceinline__ void flush_ref_counters(const Cols& C, u32 lane, u64 
     }
 }
 
+// Programmatic dependent launch (sm_90, launch_pdl): the step kernels are launched so that their CTAs may be set up
+// while the kernel before them in the stream drains; each waits here, before its first read of anything that kernel
+// wrote.  Launched without the attribute, the wait returns at once.
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+#ifdef RA_WARP_TIMELINE
+// Compile-time probe (off by default; tools/warp_timeline.py builds and reads it): every warp of raft_step_kernel
+// records where its time went, TL_WORDS words per warp, indexed by the warp's record tile:
+//   [0] SM id | leader lanes << 32 | 1 << 63 (written)   [1] tile
+//   [2..5] %globaltimer (ns) at start, inputs landed, end of the event loop, exit   [6..9] clock64 at the same points
+//   lane 0's clock64 cycles: [10] TMA issue  [11] mbarrier wait  [12] LDS + decode  [13] planes
+//   [14] peers_writeback  [15] row_end_of_step  [16] member_writeback  [17] stall list + counters
+//   [18 + 2t] handler cycles of event type t (15: lane 0 evaluated no record)   [19 + 2t] count
+#define TL_WORDS 64
+#define TL_WARPS_MAX 32768
+__device__ u64 g_tl[TL_WARPS_MAX * TL_WORDS];
+__device__ __forceinline__ u64 tl_gtime() { u64 t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+__device__ __forceinline__ u32 tl_smid() { u32 s; asm volatile("mov.u32 %0, %%smid;" : "=r"(s)); return s; }
+#define TL(...) __VA_ARGS__
+#else
+#define TL(...)
+#endif
+
 // the hot kernel, once per index width (raft_step.cuh): ra_wide::raft_step_kernel, ra_narrow::raft_step_kernel
 namespace ra_wide {
 #define RA_NARROW_PASS 0
@@ -167,6 +190,7 @@ raft_general_kernel(const __grid_constant__ Cols C, const int cur, const FloodAr
     constexpr int MM = MK_MM(0, TR_RUNTIME);
     __shared__ ulonglong2 s_peers[RA_MAX_MEMBERS * CTA_T + RA_MAX_MEMBERS * CTA_T / 2];   // nm[8][T] then cs[8][T]
     const u32 tid = threadIdx.x, lane = tid & 31u;
+    grid_dep_wait();
     if (*C.abort) return;
     const u32 n = *stall_count;
     for (u32 base = blockIdx.x * CTA_T; base < n; base += gridDim.x * CTA_T) {
@@ -839,6 +863,20 @@ extern "C" int ra_engine_load_query_state(ra_engine* e, const ra_query_state* q,
 extern "C" int ra_engine_read_query_state(ra_engine* e, ra_query_state* q, size_t n)
 { return query_io(e, q, n, false); }
 
+// a step kernel launched with programmatic stream serialisation: its CTAs may be scheduled while the kernel before
+// it in the stream drains (the kernel waits for that one in grid_dep_wait before it reads anything)
+template <typename... P, typename... A>
+static cudaError_t launch_pdl(void (*kernel)(P...), u32 grid, size_t smem, cudaStream_t s, A&&... args)
+{
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(CTA_T); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, static_cast<A&&>(args)...);
+}
+
 static int launch_step(ra_engine* e, const FloodArgs& F)
 {
     if (e->C.n_shards > 1) {
@@ -856,8 +894,9 @@ static int launch_step(ra_engine* e, const FloodArgs& F)
     u32* cnt = e->d_stall_cnt + (e->steps & 1), *cnt_next = e->d_stall_cnt + ((e->steps + 1) & 1);
     // one specialisation of the hot kernel per (member count, transport): see MK_MM
     const int tr = !e->C.routed ? TR_HOST : (e->C.n_shards > 1 ? (e->C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
-#define LAUNCH_NS(NS, NARROW, MEMB, TRN, FLT) NS::raft_step_kernel<MK_MM(MEMB, TRN), FLT><<<grid, CTA_T, sizeof(StepSmem<MK_MM(MEMB, TRN), NARROW>), e->stream>>>( \
-        e->C, e->cur, F, e->d_stall, cnt, cnt_next)
+    cudaError_t ce = cudaSuccess;
+#define LAUNCH_NS(NS, NARROW, MEMB, TRN, FLT) ce = launch_pdl(NS::raft_step_kernel<MK_MM(MEMB, TRN), FLT>, grid, \
+        sizeof(StepSmem<MK_MM(MEMB, TRN), NARROW>), e->stream, e->C, e->cur, F, e->d_stall, cnt, cnt_next)
 #define LAUNCH(MEMB, TRN, FLT) LAUNCH_NS(ra_wide, false, MEMB, TRN, FLT)
 #ifndef RA_NO_NARROW
     // 32-bit index arithmetic for the specialisations that carry the load (exact: rows or records that do not fit
@@ -888,10 +927,10 @@ static int launch_step(ra_engine* e, const FloodArgs& F)
 #undef LAUNCH
 #undef LAUNCH_N
 #undef LAUNCH_NS
-    cudaError_t ce = cudaGetLastError();
+    if (ce == cudaSuccess) ce = cudaGetLastError();
     if (ce != cudaSuccess) return fail(e, ce, "raft_step_kernel");
-    raft_general_kernel<<<e->general_grid, CTA_T, 0, e->stream>>>(e->C, e->cur, F, e->d_stall, cnt);
-    ce = cudaGetLastError();
+    ce = launch_pdl(raft_general_kernel, e->general_grid, 0, e->stream, e->C, e->cur, F, e->d_stall, cnt);
+    if (ce == cudaSuccess) ce = cudaGetLastError();
     if (ce != cudaSuccess) return fail(e, ce, "raft_general_kernel");
     if (e->C.routed) e->cur ^= 1;
     e->steps++;
@@ -1183,6 +1222,20 @@ extern "C" int ra_engine_flood_faults(ra_engine* e, uint32_t n_steps, uint32_t c
     e->last_launches = 2 * n_steps;
     return RA_OK;
 }
+
+#ifdef RA_WARP_TIMELINE
+// the probe's buffer (g_tl): out == NULL clears it, otherwise its first n_words words are copied to out
+extern "C" int ra_engine_warp_timeline(ra_engine* e, uint64_t* out, size_t n_words)
+{
+    if (!e || n_words > (size_t)TL_WARPS_MAX * TL_WORDS) return RA_E_INVAL;
+    CK(cudaSetDevice(e->cfg.device));
+    CK(cudaStreamSynchronize(e->stream));
+    if (!out) { void* p = nullptr; CK(cudaGetSymbolAddress(&p, g_tl)); CK(cudaMemset(p, 0, sizeof(g_tl))); }
+    else CK(cudaMemcpyFromSymbol(out, g_tl, n_words * sizeof(u64)));
+    CK(cudaDeviceSynchronize());
+    return RA_OK;
+}
+#endif
 
 extern "C" int ra_engine_stall_histogram(ra_engine* e, uint64_t* out128)
 {

@@ -674,9 +674,9 @@ __device__ __forceinline__ void set_fatal(Member& m, u32 code)
     MT_SET(m.meta, 26, 1, 1);
 }
 
-// out of line on purpose (scalar arguments only, nothing of the member escapes): called from many
-// places, and the hot kernel has to stay small
-__device__ __noinline__ void note_store_raw(ra_note* slot_ptr, u32 row, u32 type, u32 slot, u32 aux, u64 a, u64 b, u64 c)
+// inlined: as an out-of-line call (to keep the hot kernel small) every note cost the leader chain a call and the
+// saving of live registers around it, and the 100k x 5 flood ran ~1.7 % slower (DESIGN.md §7)
+__device__ __forceinline__ void note_store_raw(ra_note* slot_ptr, u32 row, u32 type, u32 slot, u32 aux, u64 a, u64 b, u64 c)
 {
     ulonglong2* q = reinterpret_cast<ulonglong2*>(slot_ptr);
     q[0] = make_ulonglong2((u64)row | ((u64)(type & 0xff) << 32) | ((u64)(slot & 0xff) << 40) | ((u64)(aux & 0xffff) << 48), a);
@@ -687,9 +687,9 @@ __device__ __forceinline__ void note_store(Member& m, u32 k, u32 type, u32 slot,
     note_store_raw(&m.C->onote[(size_t)k * m.C->rows + m.row], m.row, type, slot, aux, a, b, c);
 }
 
-// a host ("local") event record (RS_PLAIN) into tiled plane k; out of line for the same reason.
+// a host ("local") event record (RS_PLAIN) into tiled plane k; inlined for the same reason.
 // Returns RF_NOT_SHORT when it had to be written as a head (loc_n bit 12 + k).
-__device__ __noinline__ u32 put_local(ulonglong2* loc, u32 tiles, u32 k, u32 row, u32 type, u32 flags, u32 n, u64 term, u64 a, u64 b)
+__device__ __forceinline__ u32 put_local(ulonglong2* loc, u32 tiles, u32 k, u32 row, u32 type, u32 flags, u32 n, u64 term, u64 a, u64 b)
 {
     ulonglong2* q = loc + rec_word(tiles, k, row, 0);
     if (((term | a | b) >> 32) == 0 && rec_short_fits(type, RA_NO_SLOT, flags, n, 0)) {

@@ -14,6 +14,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     typedef StepSmem<MM, RA_NARROW_PASS != 0> Smem;
     Smem& S = *reinterpret_cast<Smem*>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    TL(__shared__ u64 tl_acc[WARPS][TL_WORDS]; const u64 tl_g0 = tl_gtime(), tl_c0 = clock64();)
 #ifdef RA_INTERLEAVE
     // CTAs are handed their tiles slot-interleaved: consecutive CTAs work on different slots' row ranges, so that
     // the long-running warps of one kind of row (a slot full of leaders) are spread over the whole launch
@@ -30,6 +31,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     const bool valid = r < C.rows;
     u32 k_events = 0, k_commits = 0, k_applied = 0, k_msgs = 0, k_dropped = 0, k_elect = 0, k_fatal = 0;
     u64 k_ref = 0;
+    grid_dep_wait();                                            // nothing of the previous kernel is read before this
     if (blockIdx.x == 0 && tid == 0) *stall_count_next = 0;    // the list of the step after this one
 
     // ---- what does this row have to do? ---------------------------------------------------
@@ -74,6 +76,9 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     mask_t todo = mask_or_warp(mine);                           // planes still to consume
     const u32 w_tail = __reduce_or_sync(0xffffffffu, my_tail);
     if (!__any_sync(0xffffffffu, work)) return;                 // whole warp idle
+    TL(const u64 tl_g1 = tl_gtime(), tl_c1 = clock64();
+       tl_acc[warp][lane] = 0; tl_acc[warp][lane + 32] = 0; __syncwarp();
+       const u32 tl_lead = __popc(__ballot_sync(0xffffffffu, valid && MT_ROLE(ap.y) == RA_LEADER));)
     u64* bars = &S.bars[warp][0];
     if (lane == 0) {
         for (int i = 0; i < NST; i++) mbar_init(&bars[i], 1);
@@ -109,6 +114,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     u32 n_issued = 0, n_done = 0, st_issue = 0, st = 0, par = 0; // ring positions = counters mod NST, phase parity
 #pragma unroll 1
     while (todo) {
+        TL(const u64 tl_a = clock64();)
         if (lane == 0) {
 #pragma unroll 1
             while (toissue && n_issued < n_done + NST) {
@@ -127,9 +133,11 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
                 n_issued++; st_issue = st_issue + 1 == NST ? 0 : st_issue + 1;
             }
         }
+        TL(const u64 tl_b = clock64();)
         const u32 p = mask_ffs(todo); todo &= todo - 1;
         const bool my = !stalled && ((mine >> p) & 1u);
         mbar_wait(&bars[st], par);
+        TL(const u64 tl_c = clock64(); u64 tl_d = tl_c; u32 tl_t = 15;)
         if (my) {
             const ulonglong2* sp = &S.stage[warp][st][0];
             const ulonglong2 c0 = sp[lane], c1 = sp[RT + lane];
@@ -137,6 +145,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
             if (rec_has_tail(c0)) { t2 = sp[2 * RT + lane]; t3 = sp[3 * RT + lane]; }
             Rec e;
             const bool fits = rec_decode(c0, c1, t2, t3, r, e);  // (narrow pass: every field below 2^30)
+            TL(tl_d = clock64(); tl_t = R_type(e) & 15u;)
             if (MT_FATAL(m.meta)) m.c_pack += 1u;
             else if (FAULTS && p < NPM && flood_lost<MM>(F, C, m, r, e)) m.c_pack += 1u << 20;   // fault injection: lost in transit
             else if (!fits || !note_budget_ok(m) || C.pure || !fast_event<MM>(m, e)) {
@@ -145,19 +154,29 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
                 atomicAdd(&C.counters[8 + (m_role(m) & 7u) * 16 + (R_type(e) & 15u)], 1ull);   // diagnostics
             }
         }
+        TL(if (lane == 0) {
+               u64* a = tl_acc[warp]; const u64 tl_e = clock64();
+               a[10] += tl_b - tl_a; a[11] += tl_c - tl_b; a[12] += tl_d - tl_c; a[13]++;
+               a[18 + 2 * tl_t] += tl_e - tl_d; a[19 + 2 * tl_t]++;
+           })
         n_done++;
         if (++st == NST) { st = 0; par ^= 1u; }
         __syncwarp();                                           // every lane is done with the slot
     }
+    TL(const u64 tl_g2 = tl_gtime(), tl_c2 = clock64(); u64 tl_t0 = 0, tl_t1 = 0, tl_t2 = 0, tl_t3 = 0;)
     const u32 rem_mbox = (u32)(rem & (((mask_t)1 << (NPM - 1) << 1) - 1)), rem_loc = (u32)(rem >> (NPM - 1) >> 1);
 
     if (work) {
         if (cntw && !fatal0) C.mbox_cnt[cur][r] = 0;
         if (nloc) C.loc_n[r] = 0;
         if ((m.pstate & 3u) == 2u) asm volatile("cp.async.wait_all;" ::: "memory");   // prefetch never consumed
+        TL(tl_t0 = clock64();)
         peers_writeback<MM>(m);
+        TL(tl_t1 = clock64();)
         if (!stalled) k_fatal = row_end_of_step<MM, FAULTS>(m, C, r, cur, F);
+        TL(tl_t2 = clock64();)
         if (!wide_row) member_writeback(m, C, r);               // (a wide row's registers were never valid here)
+        TL(tl_t3 = clock64();)
         k_events = m.c_pack & 0xffu; k_commits = m.c_commits; k_applied = m.c_applied;
         k_msgs = (m.c_pack >> 8) & 0xffu; k_dropped = m.c_pack >> 20; k_elect = (m.c_pack >> 16) & 15u;
         k_ref = m.c_ref;
@@ -179,6 +198,17 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     }
     flush_counters(C, lane, k_events, k_commits, k_applied, k_msgs, k_dropped, k_elect, k_fatal);
     flush_ref_counters(C, lane, k_ref);
+#ifdef RA_WARP_TIMELINE
+    const u64 tl_g3 = tl_gtime(), tl_c3 = clock64();
+    __syncwarp();
+    if (lane == 0 && wtile < TL_WARPS_MAX) {
+        u64* o = &g_tl[(size_t)wtile * TL_WORDS];
+        for (int i = 10; i < TL_WORDS; i++) o[i] = tl_acc[warp][i];
+        o[0] = tl_smid() | ((u64)tl_lead << 32) | (1ull << 63); o[1] = wtile;
+        o[2] = tl_g0; o[3] = tl_g1; o[4] = tl_g2; o[5] = tl_g3; o[6] = tl_c0; o[7] = tl_c1; o[8] = tl_c2; o[9] = tl_c3;
+        o[14] = tl_t1 - tl_t0; o[15] = tl_t2 - tl_t1; o[16] = tl_t3 - tl_t2; o[17] = tl_t3 ? tl_c3 - tl_t3 : 0;
+    }
+#endif
 }
 
 #undef RA_STEP_MINB
