@@ -100,7 +100,8 @@ enum ra_event_type {
  *  AER             leader      rpc term  prev_log_index  prev_log_term  leader_commit  entry term   term of the entries after the
  *                                                                                                    first n1 (used when n1 != 0)
  *                  n = number of entries (prev+1 .. prev+n); n1 = 0: all have term d, else the first
- *                  n1 have term d and the other n-n1 have term e (an AER spans <= 2 term runs)
+ *                  n1 have term d and the other n-n1 have term e (an AER spans <= 2 term runs and carries
+ *                  <= 65535 entries: a longer batch is cut, the next pipeline pass sends the rest)
  *  AER_REPLY       replier     term      next_index      last_index     last_term      success(0/1)
  *  REQUEST_VOTE    candidate   term      last_log_index  last_log_term
  *  REQUEST_VOTE_RES voter      term      -               -              -              granted(0/1)

@@ -547,6 +547,7 @@ static u64 make_append_entries_rpc(ctx_t *c, u32 peer, i64 prev_idx, u64 prev_te
     u64 last = m->log.last_index;
     u64 from = (u64)(prev_idx + 1);
     u64 to = (u64)prev_idx + num; if (last < to) to = last;              /* min(LastIndex, PrevIdx + Num) */
+    if (to >= from && to - from >= 0xFFFFu) to = from + 0xFFFEu;        /* contract: <= 65535 entries per record */
     msg_t r; memset(&r, 0, sizeof r);
     r.type = RA_EV_AER;
     r.term = m->current_term;

@@ -950,6 +950,7 @@ __device__ __forceinline__ ix_t make_aer(Member& m, u32 peer, sx_t prev_idx, ix_
     ix_t last = m.last_idx;
     ix_t from = (ix_t)(prev_idx + 1);
     ix_t to = (ix_t)prev_idx + num; if (last < to) to = last;
+    if (to >= from && to - from >= 0xFFFFu) to = from + 0xFFFEu;     // contract: <= 65535 entries per record
     u32 n = 0, n1 = 0; ix_t d = 0, e = 0;
     ix_t s = 0, t = IX_UNDEF, end = 0; u32 k = 0;
     if (to >= from && log_nonempty(m) && from <= m.last_idx) {

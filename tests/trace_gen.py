@@ -40,7 +40,20 @@ class Cluster:
         self.roles: Dict[int, int] = {}
         self.idle: Dict[int, int] = defaultdict(int)
 
-    def _post(self, e: abi.RaEvent, min_delay: int = 0) -> None:
+    def on_wal_append(self, note: abi.RaNote, written: abi.RaEvent) -> None:
+        """Called with every WAL_APPEND note and the written event made from it, before that event is queued
+        (a subclass that models the WAL's durability hooks in here; the default draws nothing)."""
+
+    def restarted(self, row: int) -> None:
+        """The member on `row` was restarted: a new process has an empty mailbox and is a follower.  Records it
+        sent before, still in flight to other rows, stay in flight."""
+        self.queues.pop(row, None)
+        self.delayed = [x for x in self.delayed if x[1].row != row]
+        self.roles[row] = abi.FOLLOWER
+        self.idle[row] = 0
+
+    def _post(self, e: abi.RaEvent, min_delay: int = 0, duplicate: bool = False) -> None:
+        """queue e for a later step; duplicate: e is the network's second copy of a record already posted"""
         d = min_delay
         while self.rng.random() < self.p_delay:
             d += 1
@@ -111,17 +124,19 @@ class Cluster:
                 continue
             self._post(copy_ev(m))
             if rng.random() < self.p_dup:
-                self._post(copy_ev(m), 1)
+                self._post(copy_ev(m), 1, duplicate=True)
         saw_leader = set()
         for i, n in enumerate(notes):
             last_of_row = i + 1 == len(notes) or notes[i + 1].row != n.row
             if last_of_row and n.type != abi.NOTE_STATUS and (n.aux & abi.ST_LEADER_MSG):
                 saw_leader.add(n.row)                      # flags riding in the row's last note
             if n.type == abi.NOTE_WAL_APPEND:
+                w = abi.ev_written(n.row, n.c, n.a, n.b)
+                self.on_wal_append(n, w)
                 if rng.random() < self.p_withhold:
-                    self._post(abi.ev_written(n.row, n.c, n.a, n.b), rng.randint(3, 12))   # lagging fsync
+                    self._post(w, rng.randint(3, 12))   # lagging fsync
                 else:
-                    self._post(abi.ev_written(n.row, n.c, n.a, n.b))
+                    self._post(w)
             elif n.type == abi.NOTE_STATUS:
                 self.roles[n.row] = (n.b >> 24) & 0xff
                 if n.aux & abi.ST_LEADER_MSG:
