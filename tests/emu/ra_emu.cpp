@@ -13,8 +13,10 @@
  * (tests/test_emu_parity.py), so a logic regression shows up before any GPU time is spent.
  *
  * Same C ABI as include/ra_engine.h with the prefix ra_emu_.  Shards: the bucket transport
- * (ra_emu_set_outbox / ra_emu_deliver); the peer transport is the same stores through other
- * base pointers and is left to the GPU tests.
+ * (ra_emu_set_outbox / ra_emu_deliver) and the peer transport (ra_emu_peer_get / ra_emu_peer_set:
+ * the step stores straight into the other shards' mailbox planes and count bytes).  The shards of
+ * one process step one after another and share the buffer parity `cur`, so a shard's stores into
+ * another's `cur ^ 1` buffer stay invisible to that shard's step: the lock step of the GPU transport.
  */
 #include <stdint.h>
 #include <stddef.h>
@@ -274,12 +276,12 @@ static void general_row(const Cols& C, int cur, const FloodArgs& F, const StallC
 static int run_step(ra_emu* e, const FloodArgs& F)
 {
     const Cols& C = e->C;
-    if (C.n_shards > 1) {
-        if (!C.outbox) return RA_E_INVAL;                       // ra_emu_set_outbox first
+    if (C.n_shards > 1 && !C.peer_mode) {
+        if (!C.outbox) return RA_E_INVAL;                       // ra_emu_set_outbox / ra_emu_peer_set first
         memset(C.out_cnt, 0, C.n_shards * sizeof(u32));
     }
     // same choice of specialisation as launch_step() in engine.cu
-    const int tr = !C.routed ? TR_HOST : (C.n_shards > 1 ? TR_BUCKET : TR_LOCAL);
+    const int tr = !C.routed ? TR_HOST : (C.n_shards > 1 ? (C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
     u32 w_tail = 0;
     for (u32 r = 0; r < C.rows; r++) {
         if ((r & (RT - 1)) == 0) w_tail = tile_sizes(C, e->cur, r);
@@ -290,6 +292,8 @@ static int run_step(ra_emu* e, const FloodArgs& F)
             // (narrow pass for the same specialisations as launch_step(); RA_STEP_WIDE=1 keeps the 64-bit pass)
             case TR_LOCAL:  stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, w_tail, ctx)
                                                 : ra_wide::step_row<MK_MM(5, TR_LOCAL)>(C, e->cur, F, r, w_tail, ctx); break;
+            case TR_PEER:   stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_PEER)>(C, e->cur, F, r, w_tail, ctx)
+                                                : ra_wide::step_row<MK_MM(5, TR_PEER)>(C, e->cur, F, r, w_tail, ctx); break;
             case TR_BUCKET: stalled = ra_wide::step_row<MK_MM(5, TR_BUCKET)>(C, e->cur, F, r, w_tail, ctx); break;
             default:        stalled = e->narrow ? ra_narrow::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, w_tail, ctx)
                                                 : ra_wide::step_row<MK_MM(5, TR_HOST)>(C, e->cur, F, r, w_tail, ctx); break;
@@ -320,6 +324,26 @@ extern "C" int ra_emu_deliver(ra_emu* e, const void* inbox, const uint32_t* coun
         const u32 n = counts[b] < cap ? counts[b] : cap;
         for (u32 i = 0; i < n; i++) deliver_record(e->C, e->cur, ld_rec(&in[(size_t)b * cap + i]));
     }
+    return RA_OK;
+}
+
+// the peer transport (engine.cu: ra_engine_peer_get / ra_engine_peer_set): host pointers in place of device ones
+extern "C" int ra_emu_peer_get(ra_emu* e, ra_peer_ptrs* out)
+{
+    if (!e || !out || !e->C.routed) return RA_E_INVAL;
+    for (int b = 0; b < 2; b++) { out->mbox[b] = e->C.mbox[b]; out->mbox_cnt[b] = e->C.mbox_cnt[b]; }
+    return RA_OK;
+}
+
+extern "C" int ra_emu_peer_set(ra_emu* e, uint32_t shard, const ra_peer_ptrs* p)
+{
+    if (!e || !p || e->C.n_shards < 2 || e->C.n_shards > 8 || shard >= e->C.n_shards) return RA_E_INVAL;
+    Cols& C = e->C;
+    for (int b = 0; b < 2; b++) { C.peer_mbox[b][shard] = (ulonglong2*)p->mbox[b]; C.peer_cnt[b][shard] = (u64*)p->mbox_cnt[b]; }
+    for (int b = 0; b < 2; b++) { C.peer_mbox[b][C.shard] = C.mbox[b]; C.peer_cnt[b][C.shard] = C.mbox_cnt[b]; }
+    bool all = true;
+    for (u32 k = 0; k < C.n_shards; k++) all = all && C.peer_mbox[0][k] && C.peer_mbox[1][k] && C.peer_cnt[0][k] && C.peer_cnt[1][k];
+    C.peer_mode = all ? 1 : 0;
     return RA_OK;
 }
 

@@ -117,19 +117,40 @@ class EmuHostFlood:
             self._h = C.c_void_p()
 
 
-class EmuShards:
-    """N emulated shards in this process with the bucket transport: the CPU twin of
-    ra_b200.sharded.Shard + LocalTransport + ShardedFlood (member (g, s) on shard (g + s) mod N)."""
+class PeerPtrs(C.Structure):
+    """ra_peer_ptrs (include/ra_engine.h)"""
+    _fields_ = [("mbox", C.c_void_p * 2), ("mbox_cnt", C.c_void_p * 2)]
 
-    def __init__(self, n_shards: int, groups_local: int, members: int, cap: int = 4096, **kw):
+
+class EmuShards:
+    """N emulated shards in this process: the CPU twin of ra_b200.sharded.Shard + LocalTransport + ShardedFlood
+    (member (g, s) on shard (g + s) mod N), or with peer=True of Shard + LocalPeerTransport: every shard stores
+    into the others' mailboxes (ra_emu_peer_set) and exchange() has nothing to do."""
+
+    def __init__(self, n_shards: int, groups_local: int, members: int, cap: int = 4096, peer: bool = False, **kw):
         l = lib()
         l.ra_emu_set_outbox.restype = C.c_int
         l.ra_emu_set_outbox.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
         l.ra_emu_deliver.restype = C.c_int
         l.ra_emu_deliver.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
-        self.n, self.gl, self.m, self.cap = n_shards, groups_local, members, cap
+        l.ra_emu_peer_get.restype = C.c_int
+        l.ra_emu_peer_get.argtypes = [C.c_void_p, C.POINTER(PeerPtrs)]
+        l.ra_emu_peer_set.restype = C.c_int
+        l.ra_emu_peer_set.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(PeerPtrs)]
+        self.n, self.gl, self.m, self.cap, self.peer = n_shards, groups_local, members, cap, peer
         self.shards = [Emu(groups_local, members, route_on_device=True, n_shards=n_shards, shard=k, **kw)
                        for k in range(n_shards)]
+        if peer:
+            ptrs = []
+            for s in self.shards:
+                p = PeerPtrs()
+                s._check(l.ra_emu_peer_get(s._h, C.byref(p)), "peer_get")
+                ptrs.append(p)
+            for k, s in enumerate(self.shards):
+                for j, p in enumerate(ptrs):
+                    if j != k:
+                        s._check(l.ra_emu_peer_set(s._h, j, C.byref(p)), "peer_set")
+            return
         self.outbox = [(abi.RaEvent * (n_shards * cap))() for _ in range(n_shards)]
         self.inbox = [(abi.RaEvent * (n_shards * cap))() for _ in range(n_shards)]
         self.out_cnt = [(C.c_uint32 * n_shards)() for _ in range(n_shards)]
@@ -138,6 +159,8 @@ class EmuShards:
             s._check(l.ra_emu_set_outbox(s._h, self.outbox[k], self.out_cnt[k], cap), "set_outbox")
 
     def exchange(self) -> None:
+        if self.peer:                                  # the stores landed during the step
+            return
         sz = C.sizeof(abi.RaEvent)
         for b in range(self.n):
             for a in range(self.n):
