@@ -14,6 +14,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <new>
+#include <type_traits>
 
 #include "raft_step.cuh"
 #include "raft_row.cuh"
@@ -174,13 +175,11 @@ namespace ra_wide {
 #include "raft_step_kernel.cuh"
 #undef RA_NARROW_PASS
 }
-#ifndef RA_NO_NARROW
 namespace ra_narrow {
 #define RA_NARROW_PASS 1
 #include "raft_step_kernel.cuh"
 #undef RA_NARROW_PASS
 }
-#endif
 
 // general path for the stalled rows of this step (one thread per list entry)
 __global__ void __launch_bounds__(CTA_T)
@@ -282,51 +281,49 @@ __global__ void read_query_kernel(const Cols C, ra_query_state* out, u32 n)
     if (i < n) read_query_row(C, out[i]);
 }
 
-// flat host batch -> per-row local slots.  err[0]: 1 = ungrouped, 2 = too many for a row, 3 = bad row
-__global__ void ingest_kernel(const Cols C, const ra_event* ev, u32 n, u32* err, const u32* sticky)
+// The two record forms of a host batch: which types each may carry, and how one record is stored as the k-th local
+// record of its row, returning its loc_n size bits for k = 0 (8 + k: tail, 12 + k: not short).
+// 64-byte ra_event: any event type, stored as it is.
+__device__ __forceinline__ bool ingest_type_ok(const ra_event& ev)
 {
-    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || *sticky) return;
-    const u32 row = ev[i].row;
-    if (row >= C.rows || ev[i].type > RA_EV_CONSISTENT_QUERY || ev[i].type == RA_EV_NONE) { atomicMax(err, 3u); return; }
-    if (i > 0 && ev[i - 1].row == row) return;                 // not the head of its run
-    u32 len = 1;
-    while (i + len < n && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
-    if (len > RA_LOCAL_CAP) { atomicMax(err, 2u); return; }
-    if (atomicCAS(&C.loc_n[row], 0u, len) != 0u) { atomicMax(err, 1u); return; }
-    u32 size = 0;                                              // loc_n bits 8 + k (tail), 12 + k (not short)
-    for (u32 k = 0; k < len; k++) {
-        const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]));
-        size |= (((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12)) << k;
-    }
-    if (size) atomicOr(&C.loc_n[row], size);
+    return ev.type <= RA_EV_CONSISTENT_QUERY && ev.type != RA_EV_NONE;
 }
-
-// the same for a batch of 32-byte host events: every record is RS_PLAIN; err 3 also for an RPC type
-__device__ __forceinline__ bool host_event_type_ok(u32 t)
+__device__ __forceinline__ u32 ingest_store(const Cols& C, u32 k, u32 row, const ra_event& ev)
 {
+    const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev));
+    return ((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12);
+}
+// 32-byte ra_host_event: host-origin types only (no RPC), every record RS_PLAIN
+__device__ __forceinline__ bool ingest_type_ok(const ra_host_event& ev)
+{
+    const u32 t = ev.type;
     return t == RA_EV_WRITTEN || t == RA_EV_COMMAND || t == RA_EV_ELECTION_TIMEOUT || t == RA_EV_AWAIT_COND_TIMEOUT ||
            t == RA_EV_PIPELINE_RPCS || t == RA_EV_TICK || t == RA_EV_CONSISTENT_QUERY;
 }
-__global__ void ingest_host_kernel(const Cols C, const ra_host_event* ev, u32 n, u32* err, const u32* sticky)
+__device__ __forceinline__ u32 ingest_store(const Cols& C, u32 k, u32 row, const ra_host_event& ev)
+{
+    const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&ev);
+    const ulonglong2 h = src[0], t = src[1];                   // {row | type<<32 | flags<<40 | n<<48, term}, {a, b}
+    const u32 type = (u32)(h.x >> 32) & 0xffu, flags = (u32)(h.x >> 40) & 0xffu, nn = (u32)(h.x >> 48);
+    return put_local(C.loc, C.tiles, k, row, type, flags, nn, h.y, t.x, t.y) << 12;
+}
+
+// flat host batch -> per-row local slots.  err[0]: 1 = ungrouped, 2 = too many for a row, 3 = bad row or type
+template <typename EV>
+__global__ void ingest_kernel(const Cols C, const EV* ev, u32 n, u32* err, const u32* sticky)
 {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || *sticky) return;
     const u32 row = ev[i].row;
-    if (row >= C.rows || !host_event_type_ok(ev[i].type)) { atomicMax(err, 3u); return; }
+    if (row >= C.rows || !ingest_type_ok(ev[i])) { atomicMax(err, 3u); return; }
     if (i > 0 && ev[i - 1].row == row) return;                 // not the head of its run
     u32 len = 1;
     while (i + len < n && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
     if (len > RA_LOCAL_CAP) { atomicMax(err, 2u); return; }
     if (atomicCAS(&C.loc_n[row], 0u, len) != 0u) { atomicMax(err, 1u); return; }
-    u32 heads = 0;
-    for (u32 k = 0; k < len; k++) {
-        const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&ev[i + k]);
-        const ulonglong2 h = src[0], t = src[1];               // {row | type<<32 | flags<<40 | n<<48, term}, {a, b}
-        const u32 type = (u32)(h.x >> 32) & 0xffu, flags = (u32)(h.x >> 40) & 0xffu, nn = (u32)(h.x >> 48);
-        heads |= put_local(C.loc, C.tiles, k, row, type, flags, nn, h.y, t.x, t.y) << (12 + k);
-    }
-    if (heads) atomicOr(&C.loc_n[row], heads);
+    u32 size = 0;
+    for (u32 k = 0; k < len; k++) size |= ingest_store(C, k, row, ev[i + k]) << k;
+    if (size) atomicOr(&C.loc_n[row], size);
 }
 
 // records that other shards sent to members of this engine -> mailbox planes of the next step.
@@ -364,66 +361,6 @@ struct OutHdr { u64 n_msgs, n_notes; u32 status, n_ext; };    // status: ingest 
 // outputs (ra_engine_fetch_output), and collect answers RA_E_PENDING for them.  Cleared once no call is in flight.
 #define ABORT_OUT_PENDING 4u
 
-// One warp per tile of 32 rows.  The warp's notes (and records) occupy one contiguous range of the output;
-// a small table in shared memory maps every output position to (lane, k), then the range is written in
-// 16-byte chunks, lane-consecutive: every store instruction of the warp is one contiguous 512-byte burst,
-// which is what makes writing straight into HOST memory (PCIe posted writes) efficient.
-// When the totals do not fit the caller's buffers (or the batch was rejected) nothing is written and the
-// per-row slots are left alone, so that ra_engine_fetch_output can gather again; a misfit also raises
-// ABORT_OUT_PENDING, so that the calls submitted behind this one do not touch those slots.
-__global__ void __launch_bounds__(128)
-gather_out_kernel(const Cols C, const u64* __restrict__ offs, ulonglong2* __restrict__ msgs, const u64 msgs_cap,
-                  ulonglong2* __restrict__ notes, const u64 notes_cap, OutHdr* hdr, u32* err)
-{
-    __shared__ unsigned short tab[4][32 * (RA_NOTE_CAP > RA_MSG_CAP ? RA_NOTE_CAP : RA_MSG_CAP)];
-    const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const u32 tile = blockIdx.x * 4 + warp;
-    const u64 total = offs[C.rows];
-    const u64 tm = total & 0xffffffffull, tn = total >> 32;
-    const u32 bad = *err;
-    const bool fits = tm <= msgs_cap && tn <= notes_cap;
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        hdr->n_msgs = tm; hdr->n_notes = tn; hdr->n_ext = 0; hdr->status = bad | (fits ? 0u : 0x100u);
-        if (!bad && !fits) *err = ABORT_OUT_PENDING;
-    }
-    if (bad || !fits) return;
-    const u32 r = tile * 32 + lane;
-    const bool valid = r < C.rows;
-    const u32 v = valid ? C.out_n[r] : 0u;
-    if (!__any_sync(0xffffffffu, v != 0)) return;
-    const u64 off = offs[valid ? r : C.rows];
-    if (v) C.out_n[r] = 0;
-    unsigned short* t = tab[warp];
-    {   // notes: 2 chunks each
-        const u32 nn = v >> 16;
-        const u64 on = off >> 32;
-        const u64 base = __shfl_sync(0xffffffffu, on, 0);
-        const u32 cnt = (u32)(__shfl_sync(0xffffffffu, on + nn, 31) - base);
-        for (u32 k = 0; k < nn; k++) t[(u32)(on - base) + k] = (unsigned short)((lane << 4) | k);
-        __syncwarp();
-        for (u32 c = lane; c < 2 * cnt; c += 32) {
-            const u32 ent = t[c >> 1];
-            const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)(ent & 15u) * C.rows + tile * 32 + (ent >> 4)]);
-            notes[(base << 1) + c] = src[c & 1u];
-        }
-        __syncwarp();
-    }
-    {   // RPC records: 4 chunks each
-        const u32 nm = v & 0xffffu;
-        const u64 om = off & 0xffffffffull;
-        const u64 base = __shfl_sync(0xffffffffu, om, 0);
-        const u32 cnt = (u32)(__shfl_sync(0xffffffffu, om + nm, 31) - base);
-        if (cnt == 0) return;
-        for (u32 k = 0; k < nm; k++) t[(u32)(om - base) + k] = (unsigned short)((lane << 4) | k);
-        __syncwarp();
-        for (u32 c = lane; c < 4 * cnt; c += 32) {
-            const u32 ent = t[c >> 2];
-            const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&C.omsg[(size_t)(ent & 15u) * C.rows + tile * 32 + (ent >> 4)]);
-            msgs[(base << 2) + c] = src[c & 3u];
-        }
-    }
-}
-
 // ---- compact note stream (ra_engine_set_note_format, include/ra_engine.h): one 16-byte unit per note ------------
 // A note {row, type, slot, aux, a, b, c} becomes {row, type', n, aux, a} when slot = 0, 0 <= b - a < 256 and c is
 // derivable: 0, or -- for WAL_APPEND -- the c of the row's previous WAL_APPEND note (bit 6 of type'), which the
@@ -458,20 +395,36 @@ __global__ void note_ext_count_kernel(const Cols C, u32* __restrict__ next)
     next[r] = nn ? (u32)__popc(note16_classify(C, r, nn, wc, cm)) : 0u;
 }
 
+// 16-byte units the notes of a call take in the caller's note buffer: an ra_note each, or in the compact stream one
+// unit each plus two per extension entry (behind the units)
+__host__ __device__ __forceinline__ u64 note_units(bool compact, u64 n_notes, u64 n_ext)
+{
+    return compact ? n_notes + 2 * n_ext : n_notes;
+}
+
+// One warp per tile of 32 rows.  The warp's notes (and records) occupy one contiguous range of the output;
+// a small table in shared memory maps every output position to (lane, k), then the range is written in
+// 16-byte chunks, lane-consecutive: every store instruction of the warp is one contiguous 512-byte burst,
+// which is what makes writing straight into HOST memory (PCIe posted writes) efficient.
+// COMPACT: notes leave as 16-byte units, extension entries behind them at xoffs (the scan of note_ext_count_kernel);
+// otherwise xoffs is unused.
+// When the totals do not fit the caller's buffers (or the batch was rejected) nothing is written and the
+// per-row slots are left alone, so that ra_engine_fetch_output can gather again; a misfit also raises
+// ABORT_OUT_PENDING, so that the calls submitted behind this one do not touch those slots.
+template <bool COMPACT>
 __global__ void __launch_bounds__(128)
-gather_out16_kernel(const Cols C, const u64* __restrict__ offs, const u32* __restrict__ xoffs,
-                    ulonglong2* __restrict__ msgs, const u64 msgs_cap, ulonglong2* __restrict__ units, const u64 units_cap,
-                    OutHdr* hdr, u32* err)
+gather_out_kernel(const Cols C, const u64* __restrict__ offs, const u32* __restrict__ xoffs,
+                  ulonglong2* __restrict__ msgs, const u64 msgs_cap, ulonglong2* __restrict__ notes, const u64 notes_cap,
+                  OutHdr* hdr, u32* err)
 {
     __shared__ unsigned short tab[4][32 * (RA_NOTE_CAP > RA_MSG_CAP ? RA_NOTE_CAP : RA_MSG_CAP)];
-    __shared__ u32 s_mask[4][32], s_xb[4][32];
     const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const u32 tile = blockIdx.x * 4 + warp;
     const u64 total = offs[C.rows];
     const u64 tm = total & 0xffffffffull, tn = total >> 32;
-    const u64 tx = xoffs[C.rows];
+    const u64 tx = COMPACT ? xoffs[C.rows] : 0;
     const u32 bad = *err;
-    const bool fits = tm <= msgs_cap && tn + 2 * tx <= units_cap;
+    const bool fits = tm <= msgs_cap && note_units(COMPACT, tn, tx) <= notes_cap;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         hdr->n_msgs = tm; hdr->n_notes = tn; hdr->n_ext = (u32)tx; hdr->status = bad | (fits ? 0u : 0x100u);
         if (!bad && !fits) *err = ABORT_OUT_PENDING;
@@ -489,44 +442,55 @@ gather_out16_kernel(const Cols C, const u64* __restrict__ offs, const u32* __res
         const u64 on = off >> 32;
         const u64 base = __shfl_sync(0xffffffffu, on, 0);
         const u32 cnt = (u32)(__shfl_sync(0xffffffffu, on + nn, 31) - base);
-        // the owner walks its row's notes in order (the WAL_APPEND rule depends on the one before)
-        u32 extmask = 0, cmask = 0;
-        const u32 xb = valid ? xoffs[r] : 0u;
-        if (nn) {
-            u64 wc = C.wc[r];
-            extmask = note16_classify(C, r, nn, wc, cmask);
-            C.wc[r] = wc;
-            for (u32 k = 0; k < nn; k++) {
-                t[(u32)(on - base) + k] = (unsigned short)((lane << 4) | k);
-                if ((extmask >> k) & 1u) {                           // {a, b}, {c, 0} into the extension area
-                    const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)k * C.rows + r]);
-                    const u64 idx = xb + (u32)__popc(extmask & ((1u << k) - 1u));
-                    units[tn + 2 * idx] = make_ulonglong2(q[0].y, q[1].x);
-                    units[tn + 2 * idx + 1] = make_ulonglong2(q[1].y, 0);
+        if constexpr (!COMPACT) {                                    // 2 chunks per note
+            for (u32 k = 0; k < nn; k++) t[(u32)(on - base) + k] = (unsigned short)((lane << 4) | k);
+            __syncwarp();
+            for (u32 c = lane; c < 2 * cnt; c += 32) {
+                const u32 ent = t[c >> 1];
+                const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)(ent & 15u) * C.rows + tile * 32 + (ent >> 4)]);
+                notes[(base << 1) + c] = src[c & 1u];
+            }
+        } else {
+            __shared__ u32 s_mask[4][32], s_xb[4][32];
+            // the owner walks its row's notes in order (the WAL_APPEND rule depends on the one before)
+            u32 extmask = 0, cmask = 0;
+            const u32 xb = valid ? xoffs[r] : 0u;
+            if (nn) {
+                u64 wc = C.wc[r];
+                extmask = note16_classify(C, r, nn, wc, cmask);
+                C.wc[r] = wc;
+                for (u32 k = 0; k < nn; k++) {
+                    t[(u32)(on - base) + k] = (unsigned short)((lane << 4) | k);
+                    if ((extmask >> k) & 1u) {                       // {a, b}, {c, 0} into the extension area
+                        const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)k * C.rows + r]);
+                        const u64 idx = xb + (u32)__popc(extmask & ((1u << k) - 1u));
+                        notes[tn + 2 * idx] = make_ulonglong2(q[0].y, q[1].x);
+                        notes[tn + 2 * idx + 1] = make_ulonglong2(q[1].y, 0);
+                    }
                 }
             }
-        }
-        s_mask[warp][lane] = extmask | (cmask << 16);
-        s_xb[warp][lane] = xb;
-        __syncwarp();
-        for (u32 j = lane; j < cnt; j += 32) {                       // one 16-byte unit per note, lane-consecutive
-            const u32 ent = t[j], src_lane = ent >> 4, k = ent & 15u;
-            const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)k * C.rows + tile * 32 + src_lane]);
-            const ulonglong2 h = q[0];
-            const u32 m = s_mask[warp][src_lane];
-            u64 w0 = h.x, w1 = h.y;
-            if ((m >> k) & 1u) {
-                w0 |= 0x80ull << 32;                                  // type' bit 7: extension; slot stays in place
-                w1 = s_xb[warp][src_lane] + (u32)__popc(m & 0xffffu & ((1u << k) - 1u));
-            } else {
-                const u64 n = q[1].x - h.y;                           // b - a < 256 goes where the (zero) slot was
-                w0 |= (n << 40) | (((m >> (16 + k)) & 1u) ? (0x40ull << 32) : 0ull);
+            s_mask[warp][lane] = extmask | (cmask << 16);
+            s_xb[warp][lane] = xb;
+            __syncwarp();
+            for (u32 j = lane; j < cnt; j += 32) {                   // one 16-byte unit per note, lane-consecutive
+                const u32 ent = t[j], src_lane = ent >> 4, k = ent & 15u;
+                const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&C.onote[(size_t)k * C.rows + tile * 32 + src_lane]);
+                const ulonglong2 h = q[0];
+                const u32 m = s_mask[warp][src_lane];
+                u64 w0 = h.x, w1 = h.y;
+                if ((m >> k) & 1u) {
+                    w0 |= 0x80ull << 32;                              // type' bit 7: extension; slot stays in place
+                    w1 = s_xb[warp][src_lane] + (u32)__popc(m & 0xffffu & ((1u << k) - 1u));
+                } else {
+                    const u64 n = q[1].x - h.y;                       // b - a < 256 goes where the (zero) slot was
+                    w0 |= (n << 40) | (((m >> (16 + k)) & 1u) ? (0x40ull << 32) : 0ull);
+                }
+                notes[base + j] = make_ulonglong2(w0, w1);
             }
-            units[base + j] = make_ulonglong2(w0, w1);
         }
         __syncwarp();
     }
-    {   // RPC records: 4 chunks each (unchanged)
+    {   // RPC records: 4 chunks each
         const u32 nm = v & 0xffffu;
         const u64 om = off & 0xffffffffull;
         const u64 base = __shfl_sync(0xffffffffu, om, 0);
@@ -609,7 +573,7 @@ struct ra_engine {
     u64* d_offs; void* d_scan_tmp; size_t scan_tmp_bytes;
     u32* d_err;                               // [0] sticky ingest error or ABORT_OUT_PENDING (= Cols::abort), [1] peer barrier timeout
     StallCtx* d_stall; u32* d_stall_cnt;      // d_stall_cnt[2]: alternating per step
-    ra_row_state* d_rows; size_t d_rows_cap;
+    unsigned char* d_stage; size_t d_stage_cap;   // per-row structs of load / read calls (stage_rows), in bytes
     float last_ms; u32 last_launches;
     u32 general_grid;
     char err[256];
@@ -660,7 +624,7 @@ extern "C" void ra_engine_destroy(ra_engine* e)
     cudaSetDevice(e->cfg.device);
     cudaStreamSynchronize(e->stream);
     for (int i = 0; i < e->n_allocs; i++) cudaFree(e->allocs[i]);
-    cudaFree(e->d_rows); cudaFree(e->d_scan_tmp); cudaFree(e->d_scan_tmp2);
+    cudaFree(e->d_stage); cudaFree(e->d_scan_tmp); cudaFree(e->d_scan_tmp2);
     for (int i = 0; i < RA_IO_SLOTS; i++) {
         IoSlot& q = e->io[i];
         cudaFree(q.d_ev); cudaFree(q.d_msgs); cudaFree(q.d_notes);
@@ -693,6 +657,43 @@ extern "C" int ra_engine_reset_empty(ra_engine* e)
     CK(cudaMemsetAsync(e->C.wc, 0, (size_t)e->C.rows * sizeof(u64), e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return RA_OK;
+}
+
+// The specialisations of the hot kernel (see MK_MM): one per (member count, transport, fault injection) that carries
+// the load, with a 32-bit index pass (ra_narrow::) for those that have one.  Any other engine runs the runtime-M
+// kernel of its fault flag (members = 0 here).  launch_step picks the entry; ra_engine_create sets every kernel's
+// dynamic shared memory.
+typedef void (*StepKernel)(Cols, int, FloodArgs, StallCtx*, u32*, u32*);
+struct StepSpec {
+    u32 members; int tr; bool faults;
+    StepKernel wide; size_t wide_smem;
+    StepKernel narrow; size_t narrow_smem;          // null: no narrow pass
+};
+template <int MEMB, int TRN, bool FAULTS, bool NARROW>
+static constexpr StepSpec step_spec()
+{
+    constexpr int MM = MK_MM(MEMB, TRN);
+    StepSpec s = { MEMB, TRN, FAULTS, ra_wide::raft_step_kernel<MM, FAULTS>, sizeof(StepSmem<MM, false>), nullptr, 0 };
+    if constexpr (NARROW) { s.narrow = ra_narrow::raft_step_kernel<MM, FAULTS>; s.narrow_smem = sizeof(StepSmem<MM, true>); }
+    return s;
+}
+static const StepSpec k_step_kernels[] = {
+    step_spec<5, TR_LOCAL, true, false>(), step_spec<7, TR_LOCAL, true, false>(), step_spec<0, TR_RUNTIME, true, false>(),
+    step_spec<5, TR_LOCAL, false, true>(), step_spec<5, TR_PEER, false, true>(), step_spec<5, TR_HOST, false, true>(),
+    step_spec<5, TR_BUCKET, false, false>(),
+    step_spec<3, TR_LOCAL, false, true>(), step_spec<7, TR_LOCAL, false, true>(),
+    step_spec<0, TR_RUNTIME, false, false>(),
+};
+
+static const StepSpec& pick_step_kernel(u32 members, int tr, bool faults)
+{
+    const StepSpec* runtime = nullptr;
+    for (const StepSpec& s : k_step_kernels) {
+        if (s.faults != faults) continue;
+        if (s.members == members && s.tr == tr) return s;
+        if (s.members == 0) runtime = &s;
+    }
+    return *runtime;
 }
 
 extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
@@ -763,19 +764,12 @@ extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
         cub::DeviceScan::ExclusiveSum(nullptr, e->scan_tmp2_bytes, e->d_next, e->d_xoffs, (int)(R + 1), e->stream);
         if ((ce = cudaMalloc(&e->d_scan_tmp2, e->scan_tmp2_bytes ? e->scan_tmp2_bytes : 16)) != cudaSuccess) { rc = fail(e, ce, "cudaMalloc scan"); goto bad; }
     }
-#define SMEM_ATTR_NS(NS, NARROW, MEMB, TRN, FLT) \
-    if ((ce = cudaFuncSetAttribute(NS::raft_step_kernel<MK_MM(MEMB, TRN), FLT>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                   (int)sizeof(StepSmem<MK_MM(MEMB, TRN), NARROW>))) != cudaSuccess) { rc = fail(e, ce, "cudaFuncSetAttribute"); goto bad; }
-#define SMEM_ATTR(MEMB, TRN, FLT) SMEM_ATTR_NS(ra_wide, false, MEMB, TRN, FLT)
-#ifndef RA_NO_NARROW
-    SMEM_ATTR_NS(ra_narrow, true, 5, TR_LOCAL, false) SMEM_ATTR_NS(ra_narrow, true, 5, TR_PEER, false) SMEM_ATTR_NS(ra_narrow, true, 5, TR_HOST, false)
-    SMEM_ATTR_NS(ra_narrow, true, 3, TR_LOCAL, false) SMEM_ATTR_NS(ra_narrow, true, 7, TR_LOCAL, false)
-#endif
-    SMEM_ATTR(0, TR_RUNTIME, true) SMEM_ATTR(0, TR_RUNTIME, false)
-    SMEM_ATTR(5, TR_LOCAL, false) SMEM_ATTR(5, TR_PEER, false) SMEM_ATTR(5, TR_BUCKET, false) SMEM_ATTR(5, TR_HOST, false)
-    SMEM_ATTR(3, TR_LOCAL, false) SMEM_ATTR(7, TR_LOCAL, false) SMEM_ATTR(5, TR_LOCAL, true) SMEM_ATTR(7, TR_LOCAL, true)
-#undef SMEM_ATTR
-#undef SMEM_ATTR_NS
+    for (const StepSpec& s : k_step_kernels) {
+        ce = cudaFuncSetAttribute(s.wide, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s.wide_smem);
+        if (ce == cudaSuccess && s.narrow)
+            ce = cudaFuncSetAttribute(s.narrow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s.narrow_smem);
+        if (ce != cudaSuccess) { rc = fail(e, ce, "cudaFuncSetAttribute"); goto bad; }
+    }
     {
         int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
@@ -802,66 +796,43 @@ static int ensure(ra_engine* e, T** p, size_t* cap, size_t need)
     return RA_OK;
 }
 
-extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
-{
-    if (!e || (!rows && n)) return RA_E_INVAL;
-    if (n == 0) return RA_OK;
-    for (size_t i = 0; i < n; i++)
-        if (rows[i].row >= e->C.rows || rows[i].n_members != e->C.members || !ra_row_state_valid(&rows[i])) return RA_E_INVAL;
-    if (e->narrow_mode == 0 && n * 2 >= e->C.rows) {            // a bulk load: which hot kernel suits this engine?
-        size_t wide = 0;
-        for (size_t i = 0; i < n; i++) wide += row_state_is_wide(rows[i], e->C.members) ? 1 : 0;
-        e->narrow = wide * 2 < n;
-    }
-    CK(cudaSetDevice(e->cfg.device));
-    int rc = ensure(e, &e->d_rows, &e->d_rows_cap, n); if (rc) return rc;
-    CK(cudaMemcpyAsync(e->d_rows, rows, n * sizeof(ra_row_state), cudaMemcpyHostToDevice, e->stream));
-    load_rows_kernel<<<nblocks(n, 128), 128, 0, e->stream>>>(e->C, e->d_rows, (u32)n);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(e->stream));
-    return RA_OK;
-}
-
-extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n)
+// An array of per-row structs (ra_row_state, ra_query_state) through the staging buffer and a per-row kernel: a load
+// (T const) only copies it in, a read also copies back what the kernel filled in.
+template <typename T>
+static int stage_rows(ra_engine* e, T* rows, size_t n, void (*kernel)(Cols, T*, u32))
 {
     if (!e || (!rows && n)) return RA_E_INVAL;
     if (n == 0) return RA_OK;
     for (size_t i = 0; i < n; i++) if (rows[i].row >= e->C.rows) return RA_E_INVAL;
     CK(cudaSetDevice(e->cfg.device));
-    int rc = ensure(e, &e->d_rows, &e->d_rows_cap, n); if (rc) return rc;
-    CK(cudaMemcpyAsync(e->d_rows, rows, n * sizeof(ra_row_state), cudaMemcpyHostToDevice, e->stream));
-    read_rows_kernel<<<nblocks(n, 128), 128, 0, e->stream>>>(e->C, e->d_rows, (u32)n);
+    const size_t bytes = n * sizeof(T);
+    int rc = ensure(e, &e->d_stage, &e->d_stage_cap, bytes); if (rc) return rc;
+    CK(cudaMemcpyAsync(e->d_stage, rows, bytes, cudaMemcpyHostToDevice, e->stream));
+    kernel<<<nblocks(n, 128), 128, 0, e->stream>>>(e->C, reinterpret_cast<T*>(e->d_stage), (u32)n);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(rows, e->d_rows, n * sizeof(ra_row_state), cudaMemcpyDeviceToHost, e->stream));
+    if (!std::is_const<T>::value) CK(cudaMemcpyAsync((void*)rows, e->d_stage, bytes, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return RA_OK;
 }
 
-static int query_io(ra_engine* e, ra_query_state* q, size_t n, bool load)
+extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
 {
-    if (!e || (!q && n)) return RA_E_INVAL;
-    if (n == 0) return RA_OK;
-    for (size_t i = 0; i < n; i++) if (q[i].row >= e->C.rows) return RA_E_INVAL;
-    CK(cudaSetDevice(e->cfg.device));
-    ra_query_state* d = nullptr;
-    CK(cudaMalloc(&d, n * sizeof(ra_query_state)));
-    cudaError_t ce = cudaMemcpyAsync(d, q, n * sizeof(ra_query_state), cudaMemcpyHostToDevice, e->stream);
-    if (ce == cudaSuccess) {
-        if (load) load_query_kernel<<<nblocks(n, 128), 128, 0, e->stream>>>(e->C, d, (u32)n);
-        else {
-            read_query_kernel<<<nblocks(n, 128), 128, 0, e->stream>>>(e->C, d, (u32)n);
-            ce = cudaMemcpyAsync(q, d, n * sizeof(ra_query_state), cudaMemcpyDeviceToHost, e->stream);
-        }
+    if (!e || (!rows && n)) return RA_E_INVAL;
+    for (size_t i = 0; i < n; i++)
+        if (rows[i].row >= e->C.rows || rows[i].n_members != e->C.members || !ra_row_state_valid(&rows[i])) return RA_E_INVAL;
+    if (e->narrow_mode == 0 && n * 2 >= e->C.rows) {       // a bulk load: which hot kernel suits this engine?
+        size_t wide = 0;
+        for (size_t i = 0; i < n; i++) wide += row_state_is_wide(rows[i], e->C.members) ? 1 : 0;
+        e->narrow = wide * 2 < n;
     }
-    if (ce == cudaSuccess) ce = cudaGetLastError();
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-    cudaFree(d);
-    return ce == cudaSuccess ? RA_OK : fail(e, ce, "query state");
+    return stage_rows(e, rows, n, load_rows_kernel);
 }
+extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n)
+{ return stage_rows(e, rows, n, read_rows_kernel); }
 extern "C" int ra_engine_load_query_state(ra_engine* e, const ra_query_state* q, size_t n)
-{ return query_io(e, const_cast<ra_query_state*>(q), n, true); }
+{ return stage_rows(e, q, n, load_query_kernel); }
 extern "C" int ra_engine_read_query_state(ra_engine* e, ra_query_state* q, size_t n)
-{ return query_io(e, q, n, false); }
+{ return stage_rows(e, q, n, read_query_kernel); }
 
 // a step kernel launched with programmatic stream serialisation: its CTAs may be scheduled while the kernel before
 // it in the stream drains (the kernel waits for that one in grid_dep_wait before it reads anything)
@@ -886,47 +857,16 @@ static int launch_step(ra_engine* e, const FloodArgs& F)
             if (c0 != cudaSuccess) return fail(e, c0, "cudaMemsetAsync out_cnt");
         }
     }
-#ifdef RA_INTERLEAVE
-    const u32 grid = (((e->C.tiles + WARPS - 1) / WARPS + e->C.members - 1) / e->C.members) * e->C.members;
-#else
     const u32 grid = (e->C.tiles + WARPS - 1) / WARPS;
-#endif
     u32* cnt = e->d_stall_cnt + (e->steps & 1), *cnt_next = e->d_stall_cnt + ((e->steps + 1) & 1);
-    // one specialisation of the hot kernel per (member count, transport): see MK_MM
     const int tr = !e->C.routed ? TR_HOST : (e->C.n_shards > 1 ? (e->C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
-    cudaError_t ce = cudaSuccess;
-#define LAUNCH_NS(NS, NARROW, MEMB, TRN, FLT) ce = launch_pdl(NS::raft_step_kernel<MK_MM(MEMB, TRN), FLT>, grid, \
-        sizeof(StepSmem<MK_MM(MEMB, TRN), NARROW>), e->stream, e->C, e->cur, F, e->d_stall, cnt, cnt_next)
-#define LAUNCH(MEMB, TRN, FLT) LAUNCH_NS(ra_wide, false, MEMB, TRN, FLT)
-#ifndef RA_NO_NARROW
-    // 32-bit index arithmetic for the specialisations that carry the load (exact: rows or records that do not fit
-    // stall to the 64-bit general kernel); RA_STEP_WIDE=1 in the environment keeps the 64-bit hot kernel
-#define LAUNCH_N(MEMB, TRN, FLT) do { if (e->narrow) LAUNCH_NS(ra_narrow, true, MEMB, TRN, FLT); else LAUNCH_NS(ra_wide, false, MEMB, TRN, FLT); } while (0)
-#else
-#define LAUNCH_N(MEMB, TRN, FLT) LAUNCH_NS(ra_wide, false, MEMB, TRN, FLT)
-#endif
     const bool faults = (F.drop | F.withhold | F.part) != 0;     // fault injection: its own specialisations
-    if (faults) {
-        if (e->C.members == 5 && tr == TR_LOCAL) LAUNCH(5, TR_LOCAL, true);
-        else if (e->C.members == 7 && tr == TR_LOCAL) LAUNCH(7, TR_LOCAL, true);
-        else LAUNCH(0, TR_RUNTIME, true);
-    } else if (e->C.members == 5) {
-        switch (tr) {
-        case TR_LOCAL:  LAUNCH_N(5, TR_LOCAL, false); break;
-        case TR_PEER:   LAUNCH_N(5, TR_PEER, false); break;
-        case TR_BUCKET: LAUNCH(5, TR_BUCKET, false); break;
-        default:        LAUNCH_N(5, TR_HOST, false); break;
-        }
-    } else if (e->C.members == 3 && tr == TR_LOCAL) {
-        LAUNCH_N(3, TR_LOCAL, false);
-    } else if (e->C.members == 7 && tr == TR_LOCAL) {
-        LAUNCH_N(7, TR_LOCAL, false);
-    } else {
-        LAUNCH(0, TR_RUNTIME, false);
-    }
-#undef LAUNCH
-#undef LAUNCH_N
-#undef LAUNCH_NS
+    const StepSpec& s = pick_step_kernel(e->C.members, tr, faults);
+    // 32-bit index arithmetic where the specialisation has it (exact: rows or records that do not fit stall to the
+    // 64-bit general kernel); RA_STEP_WIDE=1 in the environment keeps the 64-bit hot kernel
+    const bool narrow = e->narrow && s.narrow;
+    cudaError_t ce = launch_pdl(narrow ? s.narrow : s.wide, grid, narrow ? s.narrow_smem : s.wide_smem, e->stream,
+                                e->C, e->cur, F, e->d_stall, cnt, cnt_next);
     if (ce == cudaSuccess) ce = cudaGetLastError();
     if (ce != cudaSuccess) return fail(e, ce, "raft_step_kernel");
     ce = launch_pdl(raft_general_kernel, e->general_grid, 0, e->stream, e->C, e->cur, F, e->d_stall, cnt);
@@ -964,18 +904,16 @@ static int enqueue_gather(ra_engine* e, IoSlot& q)
     if (e->compact) {
         note_ext_count_kernel<<<nblocks((u64)R + 1, 256), 256, 0, e->stream>>>(e->C, e->d_next);
         CK(cub::DeviceScan::ExclusiveSum(e->d_scan_tmp2, e->scan_tmp2_bytes, e->d_next, e->d_xoffs, (int)(R + 1), e->stream));
-        gather_out16_kernel<<<nblocks(e->C.tiles, 4), 128, 0, e->stream>>>(
-            e->C, e->d_offs, e->d_xoffs, (ulonglong2*)q.d_msgs, (u64)q.msgs_cap, (ulonglong2*)q.d_notes, (u64)q.notes_cap,
-            (OutHdr*)dh, e->d_err);
-    } else
-    gather_out_kernel<<<nblocks(e->C.tiles, 4), 128, 0, e->stream>>>(
-        e->C, e->d_offs, (ulonglong2*)q.d_msgs, (u64)q.msgs_cap, (ulonglong2*)q.d_notes, (u64)q.notes_cap, (OutHdr*)dh, e->d_err);
+    }
+    (e->compact ? gather_out_kernel<true> : gather_out_kernel<false>)<<<nblocks(e->C.tiles, 4), 128, 0, e->stream>>>(
+        e->C, e->d_offs, e->compact ? e->d_xoffs : nullptr, (ulonglong2*)q.d_msgs, (u64)q.msgs_cap,
+        (ulonglong2*)q.d_notes, (u64)q.notes_cap, (OutHdr*)dh, e->d_err);
     CK(cudaGetLastError());
     // the outputs follow by DMA, sized by what the previous call produced (+ 1/16): steady streams of batches
     // produce steady amounts of output.  (A pinned destination -- ra_engine_alloc_host / ra_engine_register_host --
     // makes it a true asynchronous copy; a pageable one is staged by the driver.)
     const size_t unit = e->compact ? 16 : sizeof(ra_note);
-    const size_t pn = e->compact ? e->pred_notes + 2 * e->pred_ext : e->pred_notes;   // compact: units, extensions behind
+    const size_t pn = note_units(e->compact, e->pred_notes, e->pred_ext);
     q.copied_msgs = e->pred_msgs + e->pred_msgs / 16 + (e->pred_msgs ? 16 : 0);
     q.copied_notes = pn + pn / 16 + (pn ? 64 : 0);
     if (q.copied_msgs > q.msgs_cap) q.copied_msgs = q.msgs_cap;
@@ -1028,10 +966,10 @@ static int submit_impl(ra_engine* e, const EvSeg* segs, size_t n_segs, bool host
         e->loc_dirty = 0;
     }
     if (n_ev) {
-        if (host32) ingest_host_kernel<<<nblocks(n_ev, 256), 256, 0, e->stream>>>(
+        if (host32) ingest_kernel<<<nblocks(n_ev, 256), 256, 0, e->stream>>>(
                         e->C, reinterpret_cast<const ra_host_event*>(q.d_ev), (u32)n_ev, e->d_err, e->d_err);
-        else ingest_kernel<<<nblocks(n_ev, 256), 256, 0, e->stream>>>(e->C, reinterpret_cast<const ra_event*>(q.d_ev),
-                                                                        (u32)n_ev, e->d_err, e->d_err);
+        else ingest_kernel<<<nblocks(n_ev, 256), 256, 0, e->stream>>>(
+                        e->C, reinterpret_cast<const ra_event*>(q.d_ev), (u32)n_ev, e->d_err, e->d_err);
         CK(cudaGetLastError());
     }
     FloodArgs F; memset(&F, 0, sizeof F);
@@ -1066,7 +1004,7 @@ static int finish_slot(ra_engine* e, IoSlot& q, size_t* n_msgs, size_t* n_notes,
     }
     if (h.status & 0x100u) {                                      // nothing lost: ra_engine_fetch_output
         e->out_pending = 1; e->pend_msgs = (size_t)h.n_msgs; e->pend_notes = (size_t)h.n_notes;
-        e->last_ext = (size_t)h.n_ext;                            // compact: the units needed are n_notes + 2 * n_ext
+        e->last_ext = (size_t)h.n_ext;                            // compact: the units needed are note_units()
         // the gather raised ABORT_OUT_PENDING; with no call behind this one, lower it now (else that call's collect does)
         if (e->io_head == e->io_tail) CK(cudaMemsetAsync(e->d_err, 0, sizeof(u32), e->stream));
         return RA_E_CAPACITY;
@@ -1080,7 +1018,7 @@ static int finish_slot(ra_engine* e, IoSlot& q, size_t* n_msgs, size_t* n_notes,
     }
     {
         const size_t unit = e->compact ? 16 : sizeof(ra_note);
-        const size_t have = e->compact ? (size_t)h.n_notes + 2 * (size_t)h.n_ext : (size_t)h.n_notes;
+        const size_t have = note_units(e->compact, h.n_notes, h.n_ext);
         if (have > q.copied_notes) {
             CK(cudaMemcpyAsync((char*)q.user_notes + q.copied_notes * unit, (const char*)q.d_notes + q.copied_notes * unit,
                                (have - q.copied_notes) * unit, cudaMemcpyDeviceToHost, e->copy_stream));

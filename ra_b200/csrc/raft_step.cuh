@@ -13,12 +13,10 @@ namespace ra_wide {
 #include "raft_row_logic.cuh"
 }
 #undef RA_NARROW_PASS
-#ifndef RA_NO_NARROW
 #define RA_NARROW_PASS 1
 namespace ra_narrow {
 #include "raft_logic.cuh"
 #include "raft_row_logic.cuh"
 }
 #undef RA_NARROW_PASS
-#endif
 using namespace ra_wide;

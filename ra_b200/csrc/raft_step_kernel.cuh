@@ -15,18 +15,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
     Smem& S = *reinterpret_cast<Smem*>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     TL(__shared__ u64 tl_acc[WARPS][TL_WORDS]; const u64 tl_g0 = tl_gtime(), tl_c0 = clock64();)
-#ifdef RA_INTERLEAVE
-    // CTAs are handed their tiles slot-interleaved: consecutive CTAs work on different slots' row ranges, so that
-    // the long-running warps of one kind of row (a slot full of leaders) are spread over the whole launch
-    // instead of filling its first wave.  (grid = per * members CTAs, see launch_step)
-    u32 wtile;
-    {
-        const u32 k = C.members, per = gridDim.x / k;
-        wtile = ((blockIdx.x % k) * per + blockIdx.x / k) * WARPS + warp;
-    }
-#else
     const u32 wtile = blockIdx.x * WARPS + warp;                 // this warp's record tile
-#endif
     const u32 r = wtile * RT + lane;
     const bool valid = r < C.rows;
     u32 k_events = 0, k_commits = 0, k_applied = 0, k_msgs = 0, k_dropped = 0, k_elect = 0, k_fatal = 0;

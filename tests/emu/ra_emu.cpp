@@ -280,7 +280,7 @@ static int run_step(ra_emu* e, const FloodArgs& F)
         if (!C.outbox) return RA_E_INVAL;                       // ra_emu_set_outbox / ra_emu_peer_set first
         memset(C.out_cnt, 0, C.n_shards * sizeof(u32));
     }
-    // same choice of specialisation as launch_step() in engine.cu
+    // M = 5 picks its specialisation by transport as the table k_step_kernels in engine.cu does; other M run runtime-M
     const int tr = !C.routed ? TR_HOST : (C.n_shards > 1 ? (C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
     u32 w_tail = 0;
     for (u32 r = 0; r < C.rows; r++) {

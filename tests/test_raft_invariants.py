@@ -637,7 +637,7 @@ def test_closed_loop_with_restarts_routed(backend, m, monkeypatch):
     run_closed_loop(b, 300, 500 + m)
 
 
-# The kernel each engine case launches (ra_b200/csrc/engine.cu, launch of raft_step_kernel): routed, M = 3, 5 and 7
+# The kernel each engine case launches (ra_b200/csrc/engine.cu, table k_step_kernels): routed, M = 3, 5 and 7
 # have their own hot kernel in both passes; unrouted, only M = 5 has one (TR_HOST); every other M runs the runtime-M
 # kernel, which has no 32-bit pass -- so RA_STEP_WIDE only matters for the first two.
 CLOSED_GPU = ([(m, g, True, w) for m, g in ((3, 512), (5, 384), (7, 256)) for w in WIDTHS]

@@ -3,7 +3,7 @@
 The hot kernel fetches 512 B of a record tile when the size flags that travel with the record counts say that every
 record of it is short, 1 KB when none has a tail, and 2 KB otherwise; past that, its staging slot holds an earlier
 tile's bytes.  The flags are set by emit_msg (local and peer stores), row_end_of_step (also after a stall, from
-StallCtx::wk_hi), deliver_record, ingest_kernel, ingest_host_kernel and the flood host model.  Every case here makes
+StallCtx::wk_hi), deliver_record, both forms of ingest_kernel and the flood host model.  Every case here makes
 records of 256 or more entries (stored as 32-byte heads) and records with a tail (64-byte long form) share tiles with
 short ones, and compares the result with the oracle bit for bit: counters and raw row state, for traces and scripted
 steps also every record and note.
@@ -241,7 +241,7 @@ def test_scripted_step_mixes_every_form_in_a_tile_twin():
     assert forms[abi.EV_AER_REPLY][HEAD] > 0 and forms[abi.EV_PRE_VOTE][LONG] > 0, forms
 
 
-# ---- step_host: 32-byte host events through ingest_host_kernel, closed loop over a routed engine --------------------
+# ---- step_host: 32-byte host events through ingest_kernel<ra_host_event>, closed loop over a routed engine ---------
 def _host_loop(b, wide_values, steps=12):
     base, term = ((1 << 32) + 100, (1 << 32) + 5) if wide_values else (100, 5)
     rows = []
