@@ -36,7 +36,14 @@ struct ra_emu {
     void* allocs[96]; int n_allocs;
     int narrow, narrow_mode;                          // as engine.cu: RA_STEP_WIDE unset = auto, 0 = always narrow, 1 = never
     int out_pending;                                  // a step's outputs did not fit: they wait in the row slots
-    int sub_busy, sub_rc; size_t sub_nm, sub_nn;      // the one "submitted" call (ra_engine_submit_host shim)
+    // the split phase (ra_engine_submit / ra_engine_collect): up to two calls in flight, oldest first.  The emulation
+    // evaluates a call when it is submitted and hands its result over at collect.
+    struct { int rc; size_t nm, nn; } sub[2];
+    int sub_n;
+    int sub_abort;                                    // != 0: the status a call submitted now gets without being
+                                                      // evaluated (a call in flight was rejected, or its outputs did not
+                                                      // fit: RA_E_PENDING); cleared once no call is in flight
+    int out_held;                                     // the call whose outputs did not fit is still in flight
 };
 
 template <typename T>
@@ -349,10 +356,9 @@ extern "C" int ra_emu_peer_set(ra_emu* e, uint32_t shard, const ra_peer_ptrs* p)
 
 // scan + gather_out: per-row slots -> flat arrays ordered by (row, seq).  When they do not fit, nothing is
 // written and the slots stay: RA_E_CAPACITY with the sizes needed, the caller fetches again (engine.cu)
-extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                   ra_note* notes, size_t notes_cap, size_t* n_notes)
+static int gather_out(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                      ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
-    if (!e) return RA_E_INVAL;
     const Cols& C = e->C;
     const u32 R = C.rows;
     size_t tm = 0, tn = 0;
@@ -373,6 +379,17 @@ extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, s
     return RA_OK;
 }
 
+// ra_engine_fetch_output: nothing pending = nothing to fetch; RA_E_BUSY while calls submitted behind the one whose
+// outputs did not fit are still to be collected
+extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                                   ra_note* notes, size_t notes_cap, size_t* n_notes)
+{
+    if (!e || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
+    if (!e->out_pending) { if (n_msgs) *n_msgs = 0; if (n_notes) *n_notes = 0; return RA_OK; }
+    if (e->sub_n) return RA_E_BUSY;
+    return gather_out(e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
+}
+
 // ra_engine_pending_output: the sizes of outputs a call left in the slots (RA_E_CAPACITY), 0 / 0 otherwise
 extern "C" int ra_emu_pending_output(ra_emu* e, size_t* n_msgs, size_t* n_notes)
 {
@@ -384,12 +401,12 @@ extern "C" int ra_emu_pending_output(ra_emu* e, size_t* n_msgs, size_t* n_notes)
     return RA_OK;
 }
 
-extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
-                           ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                           ra_note* notes, size_t notes_cap, size_t* n_notes)
+// one call: ingest, the step, the gather (what submit_impl enqueues)
+static int eval_step(ra_emu* e, const ra_event* ev, size_t n_ev,
+                     ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                     ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
-    if (!e || (!ev && n_ev) || n_ev > 0x7fffffffull) return RA_E_INVAL;
-    if (e->out_pending) return RA_E_CAPACITY;                    // ra_emu_fetch_output first
+    if ((!ev && n_ev) || n_ev > 0x7fffffffull) return RA_E_INVAL;
     const Cols& C = e->C;
     const u32 R = C.rows;
     // clear_loc_kernel, and (after a flood, whose last step wrote every row's out_n) the out_n clear of submit_impl
@@ -418,14 +435,15 @@ extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
     }
     FloodArgs F; memset(&F, 0, sizeof F);
     { const int rc = run_step(e, F); if (rc) return rc; }
-    return ra_emu_fetch_output(e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
+    return gather_out(e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
 
-extern "C" int ra_emu_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
-                                ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                ra_note* notes, size_t notes_cap, size_t* n_notes)
+// the same for 32-byte host events: widened to 64-byte records, an RPC type rejects the batch
+static int eval_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
+                          ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                          ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
-    if (!e || (!ev && n_ev)) return RA_E_INVAL;
+    if (!ev && n_ev) return RA_E_INVAL;
     ra_event* w = (ra_event*)calloc(n_ev ? n_ev : 1, sizeof(ra_event));
     if (!w) return RA_E_NOMEM;
     for (size_t i = 0; i < n_ev; i++) {
@@ -435,9 +453,31 @@ extern "C" int ra_emu_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
         w[i].row = ev[i].row; w[i].type = (uint8_t)t; w[i].from_slot = RA_NO_SLOT; w[i].flags = ev[i].flags; w[i].n = ev[i].n;
         w[i].term = ev[i].term; w[i].a = ev[i].a; w[i].b = ev[i].b;
     }
-    const int rc = ra_emu_step(e, w, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
+    const int rc = eval_step(e, w, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
     free(w);
     return rc;
+}
+
+// step = submit + collect (engine.cu: step_impl): not while a submitted call waits to be collected, nor while the
+// outputs of an earlier call wait to be fetched
+extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
+                           ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                           ra_note* notes, size_t notes_cap, size_t* n_notes)
+{
+    if (!e) return RA_E_INVAL;
+    if (e->sub_n) return RA_E_BUSY;
+    if (e->out_pending) return RA_E_CAPACITY;                    // ra_emu_fetch_output first
+    return eval_step(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
+}
+
+extern "C" int ra_emu_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
+                                ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                                ra_note* notes, size_t notes_cap, size_t* n_notes)
+{
+    if (!e) return RA_E_INVAL;
+    if (e->sub_n) return RA_E_BUSY;
+    if (e->out_pending) return RA_E_CAPACITY;
+    return eval_step_host(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
 
 extern "C" int ra_emu_flood_faults(ra_emu* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
@@ -504,16 +544,30 @@ extern "C" int ra_emu_codec_roundtrip(const ra_event* in, ra_event* out, int* ha
 extern "C" int ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
                                    size_t* n_msgs, ra_note* notes, size_t notes_cap, size_t* n_notes)
 { return ra_emu_step_host((ra_emu*)e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
-/* the split-phase pair: the emulation evaluates at submit and hands the result over at collect */
-extern "C" int ra_engine_submit_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
-                                     ra_note* notes, size_t notes_cap)
+/* the split-phase calls with the two-slot contract of include/ra_engine.h: the emulation evaluates a call when it is
+ * submitted and hands the result over at collect.  A call submitted behind a rejected one gets the same status, one
+ * submitted behind a call whose outputs did not fit gets RA_E_PENDING; neither is evaluated. */
+static int submit_call(ra_emu* m, const void* ev, size_t n_ev, bool host32, ra_event* msgs, size_t msgs_cap,
+                       ra_note* notes, size_t notes_cap)
 {
-    ra_emu* m = (ra_emu*)e;
-    if (!m || m->sub_busy) return RA_E_BUSY;
-    m->sub_rc = ra_emu_step_host(m, ev, n_ev, msgs, msgs_cap, &m->sub_nm, notes, notes_cap, &m->sub_nn);
-    m->sub_busy = 1;
+    if (!m || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
+    if (m->out_pending && !m->out_held) return RA_E_CAPACITY;   // ra_engine_fetch_output first
+    if (m->sub_n >= 2) return RA_E_BUSY;
+    auto& s = m->sub[m->sub_n++];
+    s.nm = s.nn = 0;
+    if (m->sub_abort) { s.rc = m->sub_abort; return RA_OK; }
+    s.rc = host32 ? eval_step_host(m, (const ra_host_event*)ev, n_ev, msgs, msgs_cap, &s.nm, notes, notes_cap, &s.nn)
+                  : eval_step(m, (const ra_event*)ev, n_ev, msgs, msgs_cap, &s.nm, notes, notes_cap, &s.nn);
+    if (s.rc == RA_E_CAPACITY && m->out_pending) { m->sub_abort = RA_E_PENDING; m->out_held = 1; }
+    else if (s.rc) m->sub_abort = s.rc;
     return RA_OK;
 }
+extern "C" int ra_engine_submit_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
+                                     ra_note* notes, size_t notes_cap)
+{ return submit_call((ra_emu*)e, ev, n_ev, true, msgs, msgs_cap, notes, notes_cap); }
+extern "C" int ra_engine_submit(ra_engine* e, const ra_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
+                                ra_note* notes, size_t notes_cap)
+{ return submit_call((ra_emu*)e, ev, n_ev, false, msgs, msgs_cap, notes, notes_cap); }
 extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg* segs, size_t n_segs, ra_event* msgs,
                                           size_t msgs_cap, ra_note* notes, size_t notes_cap)
 {
@@ -530,9 +584,27 @@ extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg*
 extern "C" int ra_engine_collect(ra_engine* e, size_t* n_msgs, size_t* n_notes)
 {
     ra_emu* m = (ra_emu*)e;
-    if (!m || !m->sub_busy) return RA_E_INVAL;
-    m->sub_busy = 0;
-    if (n_msgs) *n_msgs = m->sub_nm;
-    if (n_notes) *n_notes = m->sub_nn;
-    return m->sub_rc;
+    if (!m || !m->sub_n) return RA_E_INVAL;                      // nothing submitted
+    const auto s = m->sub[0];
+    m->sub[0] = m->sub[1];
+    if (--m->sub_n == 0) m->sub_abort = 0;
+    if (s.rc == RA_E_CAPACITY && m->out_held) m->out_held = 0;   // the caller learns of the outputs waiting to be fetched
+    if (n_msgs) *n_msgs = s.nm;
+    if (n_notes) *n_notes = s.nn;
+    return s.rc;
 }
+
+/* ---- the rest of the ABI the dirty-NIF shim (ra_b200/csrc/ra_engine_nif.c) calls, so that it links against this
+ * emulation on the CPU tier */
+extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out) { return ra_emu_create(cfg, (ra_emu**)out); }
+extern "C" void ra_engine_destroy(ra_engine* e) { ra_emu_destroy((ra_emu*)e); }
+extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
+{ return ra_emu_load_rows((ra_emu*)e, rows, n); }
+extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n) { return ra_emu_read_rows((ra_emu*)e, rows, n); }
+extern "C" int ra_engine_reset_empty(ra_engine* e) { return ra_emu_reset_empty((ra_emu*)e); }
+extern "C" int ra_engine_counters(ra_engine* e, ra_counters* out) { return ra_emu_counters((ra_emu*)e, out); }
+extern "C" int ra_engine_fetch_output(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                                      ra_note* notes, size_t notes_cap, size_t* n_notes)
+{ return ra_emu_fetch_output((ra_emu*)e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
+extern "C" int ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes)
+{ return ra_emu_pending_output((ra_emu*)e, n_msgs, n_notes); }

@@ -1,6 +1,7 @@
-/* TEST INFRASTRUCTURE: just enough of OTP's erl_nif.h (types and prototypes, no implementation) to
- * SYNTAX-CHECK ra_b200/csrc/ra_engine_nif.c in an image without an Erlang toolchain
- * (tests/test_abi_exports.py::test_nif_shim_compiles).  It is not the real header and links to nothing. */
+/* TEST INFRASTRUCTURE: just enough of OTP's erl_nif.h (types and prototypes) to build
+ * ra_b200/csrc/ra_engine_nif.c in an image without an Erlang toolchain.  tests/test_abi_exports.py::
+ * test_nif_shim_compiles syntax-checks the shim against it; tests/nif_stub/erl_nif_stub.c implements the calls the shim
+ * makes, and tests/test_nif_shim.py runs the shim through that implementation.  It is not the real header. */
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -31,5 +32,14 @@ ERL_NIF_TERM enif_make_uint64(ErlNifEnv*, uint64_t);
 ERL_NIF_TERM enif_make_tuple2(ErlNifEnv*, ERL_NIF_TERM, ERL_NIF_TERM);
 ERL_NIF_TERM enif_make_new_map(ErlNifEnv*);
 int enif_make_map_put(ErlNifEnv*, ERL_NIF_TERM, ERL_NIF_TERM, ERL_NIF_TERM, ERL_NIF_TERM*);
+/* what the library hands the runtime: its module name, the NIF table and the load callback (as in OTP, nif_init) */
+typedef struct {
+    const char* name;
+    int num_of_funcs;
+    ErlNifFunc* funcs;
+    int (*load)(ErlNifEnv*, void**, ERL_NIF_TERM);
+} ErlNifEntry;
+ErlNifEntry* nif_init(void);
 #define ERL_NIF_INIT(MOD, FUNCS, LOAD, RELOAD, UPGRADE, UNLOAD) \
-    int ra_nif_stub_init_##MOD(void) { (void)LOAD; return (int)(sizeof(FUNCS) / sizeof(FUNCS[0])); }
+    ErlNifEntry* nif_init(void) \
+    { static ErlNifEntry entry = { #MOD, (int)(sizeof(FUNCS) / sizeof(FUNCS[0])), FUNCS, LOAD }; return &entry; }

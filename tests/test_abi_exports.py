@@ -48,8 +48,8 @@ def test_no_device_fails_loudly():
 
 
 def test_nif_shim_compiles():
-    """ra_b200/csrc/ra_engine_nif.c (the dirty-NIF shim of INTEGRATION.md) against a stub of erl_nif.h:
-    a syntax / type check only -- there is no Erlang toolchain in this image."""
+    """ra_b200/csrc/ra_engine_nif.c (the dirty-NIF shim of INTEGRATION.md) against the stub of erl_nif.h with every
+    warning an error (tests/test_nif_shim.py builds it with the stub's implementation and runs it)."""
     import subprocess
     r = subprocess.run(["gcc", "-std=c11", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-DRA_HAVE_ERL_NIF",
                         "-I" + os.path.join(ROOT, "tests", "nif_stub"),

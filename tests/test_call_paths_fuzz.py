@@ -465,7 +465,7 @@ def test_two_calls_in_flight_engine(api, pinned):
     assert cov["calls"] == 16
 
 
-TIGHT = [("emu", "plain", 1), pytest.param("engine", "plain", 1, marks=pytest.mark.gpu),
+TIGHT = [("emu", "plain", 1), ("emu", "plain", 2), pytest.param("engine", "plain", 1, marks=pytest.mark.gpu),
          pytest.param("engine", "compact", 1, marks=pytest.mark.gpu),
          pytest.param("engine", "plain", 2, marks=pytest.mark.gpu),
          pytest.param("engine", "compact", 2, marks=pytest.mark.gpu)]
@@ -481,7 +481,7 @@ def test_tight_output_buffers(backend, fmt, depth, mode):
     o, b = Oracle(G, m, **kf._kw(mode)), make_backend(backend, G, m, **kf._kw(mode))
     if fmt == "compact":
         b.set_note_format(True)
-    api = "submit" if backend == "engine" else "submit_host"      # (the emulation has the host-event pair only)
+    api = "submit" if backend == "engine" else "submit_host"      # (tests/test_nif_shim.py takes the emulation's submit)
     cov = _chain(b, o, m, G, mode, api, rng, rounds=2, steps=6, depth=depth, tight=True, compact=fmt == "compact")
     assert cov["capacity"] > 0
     if depth == 2:
