@@ -1,9 +1,10 @@
 """ctypes mirror of include/ra_engine.h (the C ABI of the batched multi-Raft engine).
 
-Everything here is layout only: constants, POD structs and a thin call wrapper that
-works for any shared library exporting the ``<prefix>_create/_step/...`` entry points
-declared in include/ra_engine.h.  The product binds it to ``libra_engine.so`` (CUDA);
-the tests bind the same wrapper to the CPU oracle to diff the two backends.
+Everything here is layout only: constants, POD structs, the signature of every entry point
+(SIGNATURES, HOST_SIGNATURES) and a thin call wrapper that works for any shared library
+exporting the ``<prefix>_create/_step/...`` entry points declared in include/ra_engine.h.
+The product binds it to ``libra_engine.so`` (CUDA); the tests bind the same wrapper to the
+CPU oracle and to the host emulation to diff the backends.
 
 Reference records mirrored: src/ra.hrl:122-169 (RPC records), src/ra.hrl:63-75
 (ra_peer_state()), src/ra_server.erl:73-112 (ra_server_state()).
@@ -188,10 +189,131 @@ class RaCounters(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+class RaHostEventSeg(C.Structure):
+    """ra_host_event_seg: one piece of a batch handed to ra_engine_submit_host_segs"""
+    _fields_ = [("ev", C.POINTER(RaHostEvent)), ("n", C.c_size_t)]
+
+
+class RaPeerPtrs(C.Structure):
+    """ra_peer_ptrs: a shard's mailbox buffers (device pointers)"""
+    _fields_ = [("mbox", C.c_void_p * 2), ("mbox_cnt", C.c_void_p * 2)]
+
+
+class RaIpcHandles(C.Structure):
+    """ra_ipc_handles: the same buffers as CUDA IPC handles"""
+    _fields_ = [("h", (C.c_ubyte * 64) * 4)]
+
+
+class RaWalWriter(C.Structure):
+    """ra_wal_writer: one writer of a WAL batch, n_ranges x {from, to}"""
+    _fields_ = [("row", C.c_uint32), ("n_ranges", C.c_uint32), ("term", C.c_uint64),
+                ("ranges", C.POINTER(C.c_uint64))]
+
+
+class RaWalResume(C.Structure):
+    """ra_wal_resume: the first range ra_wal_batch_to_events has not emitted"""
+    _fields_ = [("writer", C.c_uint32), ("range", C.c_uint32)]
+
+
 assert C.sizeof(RaEvent) == 64
 assert C.sizeof(RaHostEvent) == 32
 assert C.sizeof(RaNote) == 32
 assert C.sizeof(RaPeerInit) == 32
+
+
+# ---- the entry points of include/ra_engine.h: name -> (restype, argtypes) ----------------------------------------
+_vp, _sz, _u32, _u64, _P = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.POINTER
+# A notes buffer holds ra_note records or, in the compact format (ra_engine_set_note_format), ra_note16 units: it is
+# declared void* so that arrays of either pass.  Device buffers (outbox, inbox, their counts) are addresses too.
+_OUT = [_P(RaEvent), _sz, _P(_sz), _vp, _sz, _P(_sz)]            # msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes
+_SUBMIT_OUT = [_P(RaEvent), _sz, _vp, _sz]                       # msgs, msgs_cap, notes, notes_cap
+_FLOOD = [_vp, _u32, _u32, _u32, _u64]                           # e, n_steps, cmds_per_step, election_permille, seed
+
+SIGNATURES = {                                                   # ra_engine_<name>
+    "create": (C.c_int, [_P(RaEngineCfg), _P(_vp)]),
+    "destroy": (None, [_vp]),
+    "get_cfg": (C.c_int, [_vp, _P(RaEngineCfg)]),
+    "load_rows": (C.c_int, [_vp, _P(RaRowState), _sz]),
+    "reset_empty": (C.c_int, [_vp]),
+    "read_rows": (C.c_int, [_vp, _P(RaRowState), _sz]),
+    "load_query_state": (C.c_int, [_vp, _P(RaQueryState), _sz]),
+    "read_query_state": (C.c_int, [_vp, _P(RaQueryState), _sz]),
+    "step": (C.c_int, [_vp, _P(RaEvent), _sz, *_OUT]),
+    "pending_output": (C.c_int, [_vp, _P(_sz), _P(_sz)]),
+    "fetch_output": (C.c_int, [_vp, *_OUT]),
+    "flood": (C.c_int, _FLOOD),
+    "flood_faults": (C.c_int, [*_FLOOD, _P(RaFloodFaults)]),
+    "sync": (C.c_int, [_vp]),
+    "counters": (C.c_int, [_vp, _P(RaCounters)]),
+    "stall_histogram": (C.c_int, [_vp, _P(_u64)]),
+    "last_kernel_ms": (C.c_int, [_vp, _P(C.c_float), _P(_u32)]),
+    "set_stream": (C.c_int, [_vp, _vp]),
+    "set_outbox": (C.c_int, [_vp, _vp, _vp, _u32]),
+    "deliver": (C.c_int, [_vp, _vp, _vp, _u32]),
+    "peer_get": (C.c_int, [_vp, _P(RaPeerPtrs)]),
+    "peer_set": (C.c_int, [_vp, _u32, _P(RaPeerPtrs)]),
+    "ipc_export": (C.c_int, [_vp, _P(RaIpcHandles)]),
+    "ipc_import": (C.c_int, [_vp, _u32, _P(RaIpcHandles)]),
+    "peer_barrier": (C.c_int, [_vp]),
+    "set_flood_barrier": (C.c_int, [_vp, C.c_int]),
+    "step_host": (C.c_int, [_vp, _P(RaHostEvent), _sz, *_OUT]),
+    "submit": (C.c_int, [_vp, _P(RaEvent), _sz, *_SUBMIT_OUT]),
+    "submit_host": (C.c_int, [_vp, _P(RaHostEvent), _sz, *_SUBMIT_OUT]),
+    "submit_host_segs": (C.c_int, [_vp, _P(RaHostEventSeg), _sz, *_SUBMIT_OUT]),
+    "collect": (C.c_int, [_vp, _P(_sz), _P(_sz)]),
+    "set_note_format": (C.c_int, [_vp, C.c_int]),
+    "last_ext_count": (_sz, [_vp]),
+    "register_host": (C.c_int, [_vp, _sz]),
+    "unregister_host": (C.c_int, [_vp]),
+    "alloc_host": (_vp, [_sz]),
+    "free_host": (None, [_vp]),
+    "strerror": (C.c_char_p, [C.c_int]),
+    "last_cuda_error": (C.c_char_p, [_vp]),
+}
+
+HOST_SIGNATURES = {                                              # ra_<name>: host code of the same library
+    "hostsim_create": (C.c_int, [_vp, _P(_vp)]),
+    "hostsim_create_multi": (C.c_int, [_P(_vp), _u32, _P(_vp)]),
+    "hostsim_destroy": (None, [_vp]),
+    "hostsim_run": (C.c_int, [_vp, _u32, _u32, _u32, _u64, C.c_int]),
+    "hostsim_stats": (C.c_int, [_vp, _P(_u64), _P(_u64), _P(C.c_double), _P(_u64)]),
+    "hostsim_breakdown": (C.c_int, [_vp, _P(C.c_double), _P(C.c_double)]),
+    "notes16_expand": (_sz, [_vp, _sz, _sz, _P(_u64), _P(RaNote), _sz]),
+    "wal_batch_to_events": (_sz, [_P(RaWalWriter), _sz, _u32, _P(RaEvent), _sz, _P(RaWalResume)]),
+}
+
+
+class Binding:
+    """The entry points `<prefix>_<name>` of one library, as private ctypes function objects made from a signature
+    table on first use: a library that lacks a symbol fails only when that call is made.  Nothing is declared on the
+    CDLL's shared attributes, so what another caller assigns to `lib.<symbol>.argtypes` does not change these."""
+
+    def __init__(self, lib: C.CDLL, prefix: str, table: dict):
+        self._lib, self._prefix, self._table, self._fns = lib, prefix, table, {}
+
+    def __getattr__(self, name: str):
+        if name.startswith("_") or name not in self._table:
+            raise AttributeError(name)
+        f = self._fns.get(name)
+        if f is None:
+            f = self._fns[name] = self.make(name)
+        return f
+
+    def make(self, name: str):
+        """A new function object for `name`, with the table's signature and not shared with this binding."""
+        restype, argtypes = self._table[name]
+        return C.CFUNCTYPE(restype, *argtypes)(("%s_%s" % (self._prefix, name), self._lib))
+
+
+_bindings: dict = {}
+
+
+def bind(lib: C.CDLL, prefix: str, table: dict = SIGNATURES) -> Binding:
+    """The Binding of `lib` for `prefix` and `table`, made once per library."""
+    key = (lib, prefix, id(table))
+    if key not in _bindings:
+        _bindings[key] = Binding(lib, prefix, table)
+    return _bindings[key]
 
 
 class RaError(RuntimeError):
@@ -246,52 +368,47 @@ def set_log(s: RaRowState, entries: Sequence[Tuple[int, int]], last_written: Tup
         s.last_written_index, s.last_written_term = last_written
 
 
+def faults_arg(faults):
+    """None, or (drop_permille, withhold_permille, partition_permille, partition_steps) -> ra_flood_faults*"""
+    return None if faults is None else C.byref(RaFloodFaults(*faults))
+
+
 class Backend:
-    """Call wrapper over one implementation of the include/ra_engine.h entry points."""
+    """One implementation of the include/ra_engine.h entry points (the CUDA engine, the CPU oracle, the host
+    emulation), called through its Binding of SIGNATURES.  A subclass names the table its library follows."""
+    SIGNATURES = SIGNATURES
 
     def __init__(self, lib: C.CDLL, prefix: str, n_groups: int, n_members: int, *, device: int = 0,
                  route_on_device: bool = False, pure: bool = False, max_pipeline_count: int = 4096,
                  max_aer_batch: int = 128, n_shards: int = 1, shard: int = 0, note_cap: int = 0):
         self._lib = lib
         self._p = prefix
+        self._api = bind(lib, prefix, self.SIGNATURES)
         self.n_groups = n_groups
         self.n_members = n_members
         self.n_rows = n_groups * n_members
         self.cfg = RaEngineCfg(n_groups, n_members, max_pipeline_count, max_aer_batch, device,
                                1 if route_on_device else 0, 1 if pure else 0, n_shards, shard, note_cap)
         self._h = C.c_void_p()
-        f = self._fn("create")
-        f.restype = C.c_int
-        f.argtypes = [C.POINTER(RaEngineCfg), C.POINTER(C.c_void_p)]
-        self._check(f(C.byref(self.cfg), C.byref(self._h)), "create")
-        self._declare()
+        self._check(self._api.create(C.byref(self.cfg), C.byref(self._h)), "create")
 
     # -- plumbing -----------------------------------------------------
-    def _fn(self, name: str):
-        return getattr(self._lib, "%s_%s" % (self._p, name))
-
     def _check(self, st: int, what: str) -> None:
         if st != RA_OK:
             raise RaError(st, "%s_%s" % (self._p, what))
 
-    def _declare(self) -> None:
-        vp = C.c_void_p
-        sz = C.c_size_t
-        self._fn("destroy").restype = None
-        self._fn("destroy").argtypes = [vp]
-        for n, args in (("load_rows", [vp, C.POINTER(RaRowState), sz]),
-                        ("reset_empty", [vp]),
-                        ("read_rows", [vp, C.POINTER(RaRowState), sz]),
-                        ("step", [vp, C.POINTER(RaEvent), sz, C.POINTER(RaEvent), sz, C.POINTER(sz),
-                                  C.POINTER(RaNote), sz, C.POINTER(sz)]),
-                        ("counters", [vp, C.POINTER(RaCounters)])):
-            f = self._fn(n)
-            f.restype = C.c_int
-            f.argtypes = args
+    def _fn(self, name: str):
+        """The entry point `name` as a function object of its own, for a caller that passes the handle itself or
+        declares on it: nothing it does changes this backend's binding."""
+        return self._api.make(name)
+
+    def call(self, name: str, *args) -> None:
+        """The entry point `name` on this backend's handle; a status other than RA_OK raises RaError."""
+        self._check(getattr(self._api, name)(self._h, *args), name)
 
     def close(self) -> None:
         if self._h:
-            self._fn("destroy")(self._h)
+            self._api.destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):  # pragma: no cover
@@ -300,127 +417,142 @@ class Backend:
         except Exception:
             pass
 
-    # -- API ----------------------------------------------------------
+    # -- rows and query state -----------------------------------------
     def row_of(self, group: int, slot: int) -> int:
         return slot * self.n_groups + group
 
     def reset_empty(self) -> None:
-        self._check(self._fn("reset_empty")(self._h), "reset_empty")
+        self.call("reset_empty")
 
     def load_rows(self, rows: Sequence[RaRowState]) -> None:
-        arr = (RaRowState * len(rows))(*rows)
-        self._check(self._fn("load_rows")(self._h, arr, len(rows)), "load_rows")
+        self.call("load_rows", (RaRowState * len(rows))(*rows), len(rows))
 
-    def read_rows(self, row_ids: Iterable[int]) -> List[RaRowState]:
-        ids = list(row_ids)
+    def _read_rows(self, ids: Sequence[int]):
         arr = (RaRowState * len(ids))()
         for i, r in enumerate(ids):
             arr[i].row = r
-        self._check(self._fn("read_rows")(self._h, arr, len(ids)), "read_rows")
-        return list(arr)
+        self.call("read_rows", arr, len(ids))
+        return arr
 
-    def step_host(self, events: Sequence[RaEvent]) -> Tuple[List[RaEvent], List[RaNote]]:
-        """step() for a batch of host-origin events, handed over as 32-byte records."""
-        f = self._fn("step_host")
-        f.restype = C.c_int
-        sz = C.c_size_t
-        f.argtypes = [C.c_void_p, C.POINTER(RaHostEvent), sz, C.POINTER(RaEvent), sz, C.POINTER(sz),
-                      C.POINTER(RaNote), sz, C.POINTER(sz)]
-        n = len(events)
-        ev = (RaHostEvent * max(n, 1))(*[RaHostEvent.of(e) for e in events])
-        msgs_cap = max(64, n * RA_MSG_CAP)
-        notes_cap = max(64, n * RA_NOTE_CAP + 64)
-        if self.cfg.route_on_device and not self.cfg.pure:
-            msgs_cap, notes_cap = 1024, max(64, self.n_rows * RA_NOTE_CAP)
-        msgs = (RaEvent * msgs_cap)()
-        notes = (RaNote * notes_cap)()
-        nm, nn = sz(0), sz(0)
-        self._check(f(self._h, ev, n, msgs, msgs_cap, C.byref(nm), notes, notes_cap, C.byref(nn)), "step_host")
-        return list(msgs[: nm.value]), list(notes[: nn.value])
+    def read_rows(self, row_ids: Iterable[int]) -> List[RaRowState]:
+        return list(self._read_rows(list(row_ids)))
+
+    def rows_bytes(self, chunk: int = 65536) -> bytes:
+        """Every row as raw ra_row_state bytes, `chunk` rows per call."""
+        return b"".join(bytes(self._read_rows(range(lo, min(self.n_rows, lo + chunk))))
+                        for lo in range(0, self.n_rows, chunk))
 
     def load_query_state(self, qs: Sequence[RaQueryState]) -> None:
-        f = self._fn("load_query_state")
-        f.restype = C.c_int
-        f.argtypes = [C.c_void_p, C.POINTER(RaQueryState), C.c_size_t]
-        arr = (RaQueryState * max(len(qs), 1))(*qs)
-        self._check(f(self._h, arr, len(qs)), "load_query_state")
+        self.call("load_query_state", (RaQueryState * max(len(qs), 1))(*qs), len(qs))
 
     def read_query_state(self, row_ids: Iterable[int]) -> List[RaQueryState]:
-        f = self._fn("read_query_state")
-        f.restype = C.c_int
-        f.argtypes = [C.c_void_p, C.POINTER(RaQueryState), C.c_size_t]
         ids = list(row_ids)
         arr = (RaQueryState * max(len(ids), 1))()
         for i, r in enumerate(ids):
             arr[i].row = r
-        self._check(f(self._h, arr, len(ids)), "read_query_state")
+        self.call("read_query_state", arr, len(ids))
         return list(arr)[: len(ids)]
+
+    # -- one call: step and step_host ---------------------------------
+    def _default_caps(self, n: int) -> Tuple[int, int]:
+        """Output buffers for a batch of n events when the caller names none."""
+        if self.cfg.route_on_device and not self.cfg.pure:   # routed: RPC records never reach the host
+            return 1024, max(64, self.n_rows * RA_NOTE_CAP)
+        msgs = max(64, n * RA_MSG_CAP, min(max(n, 1) * RA_MSG_CAP + RA_MSG_CAP * 64, self.n_rows * RA_MSG_CAP))
+        touched = self.n_rows if self.cfg.route_on_device else min(self.n_rows, max(n, 1) + 64)
+        return msgs, max(64 + n * RA_NOTE_CAP, touched * RA_NOTE_CAP)
 
     def step(self, events: Sequence[RaEvent], msgs_cap: int | None = None,
              notes_cap: int | None = None) -> Tuple[List[RaEvent], List[RaNote]]:
-        n = len(events)
-        ev = (RaEvent * max(n, 1))(*events)
-        if msgs_cap is None:
-            if self.cfg.route_on_device and not self.cfg.pure:
-                msgs_cap = 1024                       # routed: RPC records never reach the host
-            else:
-                msgs_cap = min(max(n, 1) * RA_MSG_CAP + RA_MSG_CAP * 64, self.n_rows * RA_MSG_CAP)
-        if notes_cap is None:
-            touched = self.n_rows if self.cfg.route_on_device else min(self.n_rows, max(n, 1) + 64)
-            notes_cap = touched * RA_NOTE_CAP
-        msgs = (RaEvent * msgs_cap)()
-        notes = (RaNote * notes_cap)()
-        nm = C.c_size_t(0)
-        nn = C.c_size_t(0)
-        self._check(self._fn("step")(self._h, ev, n, msgs, msgs_cap, C.byref(nm), notes, notes_cap,
-                                     C.byref(nn)), "step")
+        return self._step("step", (RaEvent * max(len(events), 1))(*events), len(events), msgs_cap, notes_cap)
+
+    def step_host(self, events: Sequence[RaEvent], msgs_cap: int | None = None,
+                  notes_cap: int | None = None) -> Tuple[List[RaEvent], List[RaNote]]:
+        """step() for a batch of host-origin events, handed over as 32-byte records."""
+        return self._step("step_host", _host_events(events), len(events), msgs_cap, notes_cap)
+
+    def _step(self, name, ev, n, msgs_cap, notes_cap):
+        dm, dn = self._default_caps(n)
+        msgs_cap = dm if msgs_cap is None else msgs_cap
+        notes_cap = dn if notes_cap is None else notes_cap
+        msgs, notes = (RaEvent * msgs_cap)(), (RaNote * notes_cap)()
+        nm, nn = C.c_size_t(0), C.c_size_t(0)
+        self.call(name, ev, n, msgs, msgs_cap, C.byref(nm), notes, notes_cap, C.byref(nn))
         return list(msgs[: nm.value]), list(notes[: nn.value])
 
     # -- output capacity: a step whose outputs did not fit lost nothing (include/ra_engine.h "Capacity") --------
-    def fetch_output(self, msgs_cap: int, notes_cap: int):
-        """-> (status, n_msgs, n_notes, msgs, notes): RA_OK, or RA_E_CAPACITY with the sizes needed."""
-        f = self._fn("fetch_output")
-        sz = C.c_size_t
-        f.restype = C.c_int
-        f.argtypes = [C.c_void_p, C.POINTER(RaEvent), sz, C.POINTER(sz), C.POINTER(RaNote), sz, C.POINTER(sz)]
-        msgs = (RaEvent * max(msgs_cap, 1))()
-        notes = (RaNote * max(notes_cap, 1))()
-        nm, nn = sz(0), sz(0)
-        st = f(self._h, msgs, msgs_cap, C.byref(nm), notes, notes_cap, C.byref(nn))
+    def pending_output(self) -> Tuple[int, int]:
+        nm, nn = C.c_size_t(0), C.c_size_t(0)
+        self.call("pending_output", C.byref(nm), C.byref(nn))
+        return nm.value, nn.value
+
+    def fetch_output(self, msgs_cap: int, notes_cap: int, out=None):
+        """-> (status, n_msgs, n_notes, msgs, notes): RA_OK, or RA_E_CAPACITY with the sizes needed.
+        out: the caller's (msgs, notes) buffers, else new ones of those capacities."""
+        msgs, notes = out or _buffers(msgs_cap, notes_cap)
+        nm, nn = C.c_size_t(0), C.c_size_t(0)
+        st = self._api.fetch_output(self._h, msgs, msgs_cap, C.byref(nm), notes, notes_cap, C.byref(nn))
         if st not in (RA_OK, RA_E_CAPACITY):
             self._check(st, "fetch_output")
-        ok = st == RA_OK
-        return st, nm.value, nn.value, (list(msgs[: nm.value]) if ok else []), (list(notes[: nn.value]) if ok else [])
+        return _outputs(st, nm.value, nn.value, msgs, notes)
 
-    # -- split-phase calls (engine only) ---------------------------------------------------------------------
-    def submit(self, events: Sequence[RaEvent], msgs_cap: int, notes_cap: int):
-        """ra_engine_submit: returns the status and a ticket holding the buffers until collect()."""
-        f = self._fn("submit")
-        sz = C.c_size_t
-        f.restype = C.c_int
-        f.argtypes = [C.c_void_p, C.POINTER(RaEvent), sz, C.POINTER(RaEvent), sz, C.POINTER(RaNote), sz]
-        n = len(events)
-        ev = (RaEvent * max(n, 1))(*events)
-        msgs = (RaEvent * max(msgs_cap, 1))()
-        notes = (RaNote * max(notes_cap, 1))()
-        st = f(self._h, ev, n, msgs, msgs_cap, notes, notes_cap)
-        return st, (ev, msgs, notes)
+    # -- split-phase calls: submit returns the status and a ticket holding the buffers until collect() ----------
+    def submit(self, events: Sequence[RaEvent], msgs_cap: int, notes_cap: int, out=None):
+        return self._submit("submit", (RaEvent * max(len(events), 1))(*events), len(events), msgs_cap, notes_cap, out)
+
+    def submit_host(self, events: Sequence[RaEvent], msgs_cap: int, notes_cap: int, out=None):
+        return self._submit("submit_host", _host_events(events), len(events), msgs_cap, notes_cap, out)
+
+    def submit_host_segs(self, parts: Sequence[Sequence[RaEvent]], msgs_cap: int, notes_cap: int, out=None):
+        """The batch handed over in pieces, one buffer per piece (the segments keep the pieces alive)."""
+        segs = (RaHostEventSeg * max(len(parts), 1))(*[RaHostEventSeg(_host_events(p), len(p)) for p in parts])
+        return self._submit("submit_host_segs", segs, len(parts), msgs_cap, notes_cap, out)
+
+    def _submit(self, name, ev, n, msgs_cap, notes_cap, out):
+        msgs, notes = out or _buffers(msgs_cap, notes_cap)
+        return getattr(self._api, name)(self._h, ev, n, msgs, msgs_cap, notes, notes_cap), (ev, msgs, notes)
 
     def collect(self, ticket):
-        f = self._fn("collect")
-        sz = C.c_size_t
-        f.restype = C.c_int
-        f.argtypes = [C.c_void_p, C.POINTER(sz), C.POINTER(sz)]
-        nm, nn = sz(0), sz(0)
-        st = f(self._h, C.byref(nm), C.byref(nn))
+        """-> (status, n_msgs, n_notes, msgs, notes) of the oldest call submitted"""
+        nm, nn = C.c_size_t(0), C.c_size_t(0)
+        st = self._api.collect(self._h, C.byref(nm), C.byref(nn))
         _ev, msgs, notes = ticket
-        ok = st == RA_OK
-        return st, nm.value, nn.value, (list(msgs[: nm.value]) if ok else []), (list(notes[: nn.value]) if ok else [])
+        return _outputs(st, nm.value, nn.value, msgs, notes)
+
+    # -- the device-side flood and what it counts ---------------------
+    def flood(self, n_steps: int, cmds_per_step: int = 1, election_permille: int = 0, seed: int = 1,
+              faults=None) -> None:
+        """faults: None or (drop_permille, withhold_permille, partition_permille, partition_steps)"""
+        self.call("flood_faults", n_steps, cmds_per_step, election_permille, seed, faults_arg(faults))
 
     def counters(self) -> dict:
         c = RaCounters()
-        self._check(self._fn("counters")(self._h, C.byref(c)), "counters")
+        self.call("counters", C.byref(c))
         return c.as_dict()
+
+    def get_cfg(self) -> RaEngineCfg:
+        cfg = RaEngineCfg()
+        self.call("get_cfg", C.byref(cfg))
+        return cfg
+
+    def stall_histogram(self) -> dict:
+        """{(role, event_type): count} of events that took the general kernel."""
+        arr = (C.c_uint64 * 128)()
+        self.call("stall_histogram", arr)
+        return {(i // 16, i % 16): int(v) for i, v in enumerate(arr) if v}
+
+
+def _host_events(events: Sequence[RaEvent]):
+    return (RaHostEvent * max(len(events), 1))(*[RaHostEvent.of(e) for e in events])
+
+
+def _buffers(msgs_cap: int, notes_cap: int):
+    return (RaEvent * max(msgs_cap, 1))(), (RaNote * max(notes_cap, 1))()
+
+
+def _outputs(st, nm, nn, msgs, notes):
+    ok = st == RA_OK
+    return st, nm, nn, (list(msgs[:nm]) if ok else []), (list(notes[:nn]) if ok else [])
 
 
 # ---- constructors for the wire records (ra.hrl record -> 64-byte record) -----------

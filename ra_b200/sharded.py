@@ -22,7 +22,7 @@ from typing import List, Sequence
 import torch
 
 from . import abi
-from .engine import Engine, lib
+from .engine import Engine
 
 import ctypes as C
 
@@ -60,37 +60,11 @@ def _multiplier(total: int) -> int:
     return a
 
 
-def _declare(l):
-    l.ra_engine_set_stream.restype = C.c_int
-    l.ra_engine_set_stream.argtypes = [C.c_void_p, C.c_void_p]
-    l.ra_engine_set_outbox.restype = C.c_int
-    l.ra_engine_set_outbox.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
-    l.ra_engine_deliver.restype = C.c_int
-    l.ra_engine_deliver.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
-    for n in ("ra_engine_peer_get", "ra_engine_ipc_export"):
-        getattr(l, n).restype = C.c_int
-        getattr(l, n).argtypes = [C.c_void_p, C.c_void_p]
-    l.ra_engine_peer_barrier.restype = C.c_int
-    l.ra_engine_peer_barrier.argtypes = [C.c_void_p]
-    for n in ("ra_engine_peer_set", "ra_engine_ipc_import"):
-        getattr(l, n).restype = C.c_int
-        getattr(l, n).argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
-
-
-class PeerPtrs(C.Structure):
-    _fields_ = [("mbox", C.c_void_p * 2), ("mbox_cnt", C.c_void_p * 2)]
-
-
-class IpcHandles(C.Structure):
-    _fields_ = [("h", (C.c_ubyte * 64) * 4)]
-
-
 class Shard:
     """One shard = one engine + its exchange buffers (torch tensors on the engine's device)."""
 
     def __init__(self, groups_local: int, members: int, n_shards: int, shard: int, device: int = 0,
                  cap: int | None = None, buckets: bool = True, **kw):
-        _declare(lib())
         self.n_shards, self.shard, self.dev = n_shards, shard, device
         self.eng = Engine(groups_local, members, device=device, route_on_device=True, n_shards=n_shards,
                           shard=shard, **kw)
@@ -103,39 +77,35 @@ class Shard:
         with torch.cuda.device(tdev):
             stream = torch.cuda.current_stream(tdev).cuda_stream
         e = self.eng
-        e._check(lib().ra_engine_set_stream(e._h, C.c_void_p(stream)), "set_stream")
+        e.call("set_stream", C.c_void_p(stream))
         if buckets:                      # bucket + all-to-all transport; not needed for peer stores
             self.outbox = torch.zeros((n_shards, self.cap, 64), dtype=torch.uint8, device=tdev)
             self.inbox = torch.zeros((n_shards, self.cap, 64), dtype=torch.uint8, device=tdev)
             self.out_cnt = torch.zeros(n_shards, dtype=torch.int32, device=tdev)
             self.in_cnt = torch.zeros(n_shards, dtype=torch.int32, device=tdev)
-            e._check(lib().ra_engine_set_outbox(e._h, C.c_void_p(self.outbox.data_ptr()),
-                                                C.c_void_p(self.out_cnt.data_ptr()), self.cap), "set_outbox")
+            e.call("set_outbox", self.outbox.data_ptr(), self.out_cnt.data_ptr(), self.cap)
 
-    def peer_ptrs(self) -> "PeerPtrs":
-        p = PeerPtrs()
-        self.eng._check(lib().ra_engine_peer_get(self.eng._h, C.byref(p)), "peer_get")
+    def peer_ptrs(self) -> abi.RaPeerPtrs:
+        p = abi.RaPeerPtrs()
+        self.eng.call("peer_get", C.byref(p))
         return p
 
-    def peer_set(self, shard: int, p: "PeerPtrs") -> None:
-        self.eng._check(lib().ra_engine_peer_set(self.eng._h, shard, C.byref(p)), "peer_set")
+    def peer_set(self, shard: int, p: abi.RaPeerPtrs) -> None:
+        self.eng.call("peer_set", shard, C.byref(p))
 
     def ipc_export(self) -> bytes:
-        h = IpcHandles()
-        self.eng._check(lib().ra_engine_ipc_export(self.eng._h, C.byref(h)), "ipc_export")
+        h = abi.RaIpcHandles()
+        self.eng.call("ipc_export", C.byref(h))
         return bytes(h)
 
     def ipc_import(self, shard: int, raw: bytes) -> None:
-        h = IpcHandles.from_buffer_copy(raw)
-        self.eng._check(lib().ra_engine_ipc_import(self.eng._h, shard, C.byref(h)), "ipc_import")
+        self.eng.call("ipc_import", shard, C.byref(abi.RaIpcHandles.from_buffer_copy(raw)))
 
     def peer_barrier(self) -> None:
-        self.eng._check(lib().ra_engine_peer_barrier(self.eng._h), "peer_barrier")
+        self.eng.call("peer_barrier")
 
     def deliver(self) -> None:
-        e = self.eng
-        e._check(lib().ra_engine_deliver(e._h, C.c_void_p(self.inbox.data_ptr()),
-                                         C.c_void_p(self.in_cnt.data_ptr()), self.cap), "deliver")
+        self.eng.call("deliver", self.inbox.data_ptr(), self.in_cnt.data_ptr(), self.cap)
 
     def bootstrap_events(self) -> List[abi.RaEvent]:
         """election_timeout for the slot-0 member of every group that lives here."""
@@ -229,10 +199,7 @@ class NvlinkPeerTransport:
         self._tok = torch.zeros(1, dtype=torch.int32, device=torch.device("cuda", shard.dev))
         # with the device barrier a multi-step flood needs no host between steps: ra_engine_flood appends it
         self.fused = bool(self.device_barrier)
-        l = lib()
-        l.ra_engine_set_flood_barrier.restype = C.c_int
-        l.ra_engine_set_flood_barrier.argtypes = [C.c_void_p, C.c_int]
-        shard.eng._check(l.ra_engine_set_flood_barrier(shard.eng._h, 1 if self.fused else 0), "set_flood_barrier")
+        shard.eng.call("set_flood_barrier", 1 if self.fused else 0)
         dist.barrier()
 
     def exchange(self) -> None:

@@ -12,9 +12,11 @@
  * library is that the CPU test tier diffs the very source the GPU runs against the oracle
  * (tests/test_emu_parity.py), so a logic regression shows up before any GPU time is spent.
  *
- * Same C ABI as include/ra_engine.h with the prefix ra_emu_.  Shards: the bucket transport
- * (ra_emu_set_outbox / ra_emu_deliver) and the peer transport (ra_emu_peer_get / ra_emu_peer_set:
- * the step stores straight into the other shards' mailbox planes and count bytes).  The shards of
+ * The C ABI of include/ra_engine.h under the header's names, so that the product's host-side callers
+ * (host_flood.cu, the dirty-NIF shim) link against it; only the emulation's own calls are ra_emu_*.
+ * Shards: the bucket transport (ra_engine_set_outbox / ra_engine_deliver) and the peer transport
+ * (ra_engine_peer_get / ra_engine_peer_set: the step stores straight into the other shards' mailbox
+ * planes and count bytes).  The shards of
  * one process step one after another and share the buffer parity `cur`, so a shard's stores into
  * another's `cur ^ 1` buffer stay invisible to that shard's step: the lock step of the GPU transport.
  */
@@ -28,7 +30,7 @@
 #include "../../ra_b200/csrc/raft_step.cuh"
 #include "../../ra_b200/csrc/raft_row.cuh"
 
-struct ra_emu {
+struct ra_engine {
     ra_engine_cfg cfg;
     Cols C;
     int cur;
@@ -47,7 +49,7 @@ struct ra_emu {
 };
 
 template <typename T>
-static int halloc(ra_emu* e, T** p, size_t count)
+static int halloc(ra_engine* e, T** p, size_t count)
 {
     void* q = calloc(count ? count : 1, sizeof(T));
     if (!q) return RA_E_NOMEM;
@@ -56,14 +58,14 @@ static int halloc(ra_emu* e, T** p, size_t count)
     return RA_OK;
 }
 
-extern "C" void ra_emu_destroy(ra_emu* e)
+extern "C" void ra_engine_destroy(ra_engine* e)
 {
     if (!e) return;
     for (int i = 0; i < e->n_allocs; i++) free(e->allocs[i]);
     free(e);
 }
 
-extern "C" int ra_emu_reset_empty(ra_emu* e)
+extern "C" int ra_engine_reset_empty(ra_engine* e)
 {
     if (!e) return RA_E_INVAL;
     for (u32 r = 0; r < e->C.rows; r++) reset_row(e->C, r);
@@ -74,12 +76,12 @@ extern "C" int ra_emu_reset_empty(ra_emu* e)
     return RA_OK;
 }
 
-extern "C" int ra_emu_create(const ra_engine_cfg* cfg, ra_emu** out)
+extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
 {
     if (!cfg || !out || cfg->n_members < 1 || cfg->n_members > RA_MAX_MEMBERS || cfg->n_groups == 0) return RA_E_INVAL;
     if ((u64)cfg->n_groups * cfg->n_members > 0x7fffffffull) return RA_E_INVAL;
     if (cfg->n_shards > 1 && (!cfg->route_on_device || cfg->shard >= cfg->n_shards || cfg->n_shards > 64)) return RA_E_INVAL;
-    ra_emu* e = (ra_emu*)calloc(1, sizeof(ra_emu));
+    ra_engine* e = (ra_engine*)calloc(1, sizeof(ra_engine));
     if (!e) return RA_E_NOMEM;
     e->cfg = *cfg;
     { const char* w = getenv("RA_STEP_WIDE"); e->narrow_mode = !(w && *w) ? 0 : (*w == '0' ? 1 : 2); e->narrow = e->narrow_mode != 2; }
@@ -115,22 +117,22 @@ extern "C" int ra_emu_create(const ra_engine_cfg* cfg, ra_emu** out)
         }
     }
 #undef HA
-    if ((rc = ra_emu_reset_empty(e)) != RA_OK) goto bad;
+    if ((rc = ra_engine_reset_empty(e)) != RA_OK) goto bad;
     *out = e;
     return RA_OK;
 bad:
-    ra_emu_destroy(e);
+    ra_engine_destroy(e);
     return rc;
 }
 
-extern "C" int ra_emu_get_cfg(ra_emu* e, ra_engine_cfg* out)
+extern "C" int ra_engine_get_cfg(ra_engine* e, ra_engine_cfg* out)
 {
     if (!e || !out) return RA_E_INVAL;
     *out = e->cfg;
     return RA_OK;
 }
 
-extern "C" int ra_emu_load_rows(ra_emu* e, const ra_row_state* rows, size_t n)
+extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
 {
     if (!e || (!rows && n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++)
@@ -144,7 +146,7 @@ extern "C" int ra_emu_load_rows(ra_emu* e, const ra_row_state* rows, size_t n)
     return RA_OK;
 }
 
-extern "C" int ra_emu_read_rows(ra_emu* e, ra_row_state* rows, size_t n)
+extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n)
 {
     if (!e || (!rows && n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) if (rows[i].row >= e->C.rows) return RA_E_INVAL;
@@ -152,7 +154,7 @@ extern "C" int ra_emu_read_rows(ra_emu* e, ra_row_state* rows, size_t n)
     return RA_OK;
 }
 
-extern "C" int ra_emu_load_query_state(ra_emu* e, const ra_query_state* q, size_t n)
+extern "C" int ra_engine_load_query_state(ra_engine* e, const ra_query_state* q, size_t n)
 {
     if (!e || (!q && n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) if (q[i].row >= e->C.rows) return RA_E_INVAL;
@@ -160,7 +162,7 @@ extern "C" int ra_emu_load_query_state(ra_emu* e, const ra_query_state* q, size_
     return RA_OK;
 }
 
-extern "C" int ra_emu_read_query_state(ra_emu* e, ra_query_state* q, size_t n)
+extern "C" int ra_engine_read_query_state(ra_engine* e, ra_query_state* q, size_t n)
 {
     if (!e || (!q && n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) if (q[i].row >= e->C.rows) return RA_E_INVAL;
@@ -280,11 +282,11 @@ static void general_row(const Cols& C, int cur, const FloodArgs& F, const StallC
     ra_wide::add_counters(C, m, k_fatal);
 }
 
-static int run_step(ra_emu* e, const FloodArgs& F)
+static int run_step(ra_engine* e, const FloodArgs& F)
 {
     const Cols& C = e->C;
     if (C.n_shards > 1 && !C.peer_mode) {
-        if (!C.outbox) return RA_E_INVAL;                       // ra_emu_set_outbox / ra_emu_peer_set first
+        if (!C.outbox) return RA_E_INVAL;                       // ra_engine_set_outbox / ra_engine_peer_set first
         memset(C.out_cnt, 0, C.n_shards * sizeof(u32));
     }
     // M = 5 picks its specialisation by transport as the table k_step_kernels in engine.cu does; other M run runtime-M
@@ -315,14 +317,14 @@ static int run_step(ra_emu* e, const FloodArgs& F)
     return RA_OK;
 }
 
-extern "C" int ra_emu_set_outbox(ra_emu* e, void* outbox, uint32_t* counts, uint32_t cap)
+extern "C" int ra_engine_set_outbox(ra_engine* e, void* outbox, uint32_t* counts, uint32_t cap)
 {
     if (!e || e->C.n_shards < 2 || !outbox || !counts || !cap) return RA_E_INVAL;
     e->C.outbox = (ra_event*)outbox; e->C.out_cnt = counts; e->C.out_cap = cap;
     return RA_OK;
 }
 
-extern "C" int ra_emu_deliver(ra_emu* e, const void* inbox, const uint32_t* counts, uint32_t cap)
+extern "C" int ra_engine_deliver(ra_engine* e, const void* inbox, const uint32_t* counts, uint32_t cap)
 {
     if (!e || e->C.n_shards < 2 || !inbox || !counts || !cap) return RA_E_INVAL;
     const ra_event* in = (const ra_event*)inbox;
@@ -335,14 +337,14 @@ extern "C" int ra_emu_deliver(ra_emu* e, const void* inbox, const uint32_t* coun
 }
 
 // the peer transport (engine.cu: ra_engine_peer_get / ra_engine_peer_set): host pointers in place of device ones
-extern "C" int ra_emu_peer_get(ra_emu* e, ra_peer_ptrs* out)
+extern "C" int ra_engine_peer_get(ra_engine* e, ra_peer_ptrs* out)
 {
     if (!e || !out || !e->C.routed) return RA_E_INVAL;
     for (int b = 0; b < 2; b++) { out->mbox[b] = e->C.mbox[b]; out->mbox_cnt[b] = e->C.mbox_cnt[b]; }
     return RA_OK;
 }
 
-extern "C" int ra_emu_peer_set(ra_emu* e, uint32_t shard, const ra_peer_ptrs* p)
+extern "C" int ra_engine_peer_set(ra_engine* e, uint32_t shard, const ra_peer_ptrs* p)
 {
     if (!e || !p || e->C.n_shards < 2 || e->C.n_shards > 8 || shard >= e->C.n_shards) return RA_E_INVAL;
     Cols& C = e->C;
@@ -356,7 +358,7 @@ extern "C" int ra_emu_peer_set(ra_emu* e, uint32_t shard, const ra_peer_ptrs* p)
 
 // scan + gather_out: per-row slots -> flat arrays ordered by (row, seq).  When they do not fit, nothing is
 // written and the slots stay: RA_E_CAPACITY with the sizes needed, the caller fetches again (engine.cu)
-static int gather_out(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+static int gather_out(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
                       ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
     const Cols& C = e->C;
@@ -381,8 +383,8 @@ static int gather_out(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs
 
 // ra_engine_fetch_output: nothing pending = nothing to fetch; RA_E_BUSY while calls submitted behind the one whose
 // outputs did not fit are still to be collected
-extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                   ra_note* notes, size_t notes_cap, size_t* n_notes)
+extern "C" int ra_engine_fetch_output(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                                      ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
     if (!e || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
     if (!e->out_pending) { if (n_msgs) *n_msgs = 0; if (n_notes) *n_notes = 0; return RA_OK; }
@@ -391,7 +393,7 @@ extern "C" int ra_emu_fetch_output(ra_emu* e, ra_event* msgs, size_t msgs_cap, s
 }
 
 // ra_engine_pending_output: the sizes of outputs a call left in the slots (RA_E_CAPACITY), 0 / 0 otherwise
-extern "C" int ra_emu_pending_output(ra_emu* e, size_t* n_msgs, size_t* n_notes)
+extern "C" int ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes)
 {
     if (!e) return RA_E_INVAL;
     size_t tm = 0, tn = 0;
@@ -402,7 +404,7 @@ extern "C" int ra_emu_pending_output(ra_emu* e, size_t* n_msgs, size_t* n_notes)
 }
 
 // one call: ingest, the step, the gather (what submit_impl enqueues)
-static int eval_step(ra_emu* e, const ra_event* ev, size_t n_ev,
+static int eval_step(ra_engine* e, const ra_event* ev, size_t n_ev,
                      ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
                      ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
@@ -439,7 +441,7 @@ static int eval_step(ra_emu* e, const ra_event* ev, size_t n_ev,
 }
 
 // the same for 32-byte host events: widened to 64-byte records, an RPC type rejects the batch
-static int eval_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
+static int eval_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev,
                           ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
                           ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
@@ -460,19 +462,19 @@ static int eval_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
 
 // step = submit + collect (engine.cu: step_impl): not while a submitted call waits to be collected, nor while the
 // outputs of an earlier call wait to be fetched
-extern "C" int ra_emu_step(ra_emu* e, const ra_event* ev, size_t n_ev,
-                           ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                           ra_note* notes, size_t notes_cap, size_t* n_notes)
+extern "C" int ra_engine_step(ra_engine* e, const ra_event* ev, size_t n_ev,
+                              ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                              ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
     if (!e) return RA_E_INVAL;
     if (e->sub_n) return RA_E_BUSY;
-    if (e->out_pending) return RA_E_CAPACITY;                    // ra_emu_fetch_output first
+    if (e->out_pending) return RA_E_CAPACITY;                    // ra_engine_fetch_output first
     return eval_step(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
 
-extern "C" int ra_emu_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
-                                ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                ra_note* notes, size_t notes_cap, size_t* n_notes)
+extern "C" int ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev,
+                                   ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                                   ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
     if (!e) return RA_E_INVAL;
     if (e->sub_n) return RA_E_BUSY;
@@ -480,13 +482,11 @@ extern "C" int ra_emu_step_host(ra_emu* e, const ra_host_event* ev, size_t n_ev,
     return eval_step_host(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
 
-extern "C" int ra_emu_flood_faults(ra_emu* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
-                                   uint64_t seed, const ra_flood_faults* ff);
-extern "C" int ra_emu_flood(ra_emu* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
-                            uint64_t seed)
-{ return ra_emu_flood_faults(e, n_steps, cmds_per_step, election_permille, seed, nullptr); }
-extern "C" int ra_emu_flood_faults(ra_emu* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
-                                   uint64_t seed, const ra_flood_faults* ff)
+extern "C" int ra_engine_flood(ra_engine* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
+                               uint64_t seed)
+{ return ra_engine_flood_faults(e, n_steps, cmds_per_step, election_permille, seed, nullptr); }
+extern "C" int ra_engine_flood_faults(ra_engine* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
+                                      uint64_t seed, const ra_flood_faults* ff)
 {
     if (!e || !e->C.routed) return RA_E_INVAL;
     if (ff && ff->partition_permille && !ff->partition_steps) return RA_E_INVAL;
@@ -502,7 +502,7 @@ extern "C" int ra_emu_flood_faults(ra_emu* e, uint32_t n_steps, uint32_t cmds_pe
     return RA_OK;
 }
 
-extern "C" int ra_emu_counters(ra_emu* e, ra_counters* out)
+extern "C" int ra_engine_counters(ra_engine* e, ra_counters* out)
 {
     if (!e || !out) return RA_E_INVAL;
     const u64* h = e->C.counters;
@@ -514,20 +514,12 @@ extern "C" int ra_emu_counters(ra_emu* e, ra_counters* out)
     return RA_OK;
 }
 
-extern "C" int ra_emu_stall_histogram(ra_emu* e, uint64_t* out128)
+extern "C" int ra_engine_stall_histogram(ra_engine* e, uint64_t* out128)
 {
     if (!e || !out128) return RA_E_INVAL;
     memcpy(out128, e->C.counters + 8, 128 * sizeof(u64));
     return RA_OK;
 }
-
-/* ---- ra_hostsim (ra_b200/csrc/host_flood.cu, the host-side caller of the ABI used by the e2e
- * benchmark) over this emulation: the file is compiled into this library with RA_NO_CUDA and
- * reaches the "engine" through these three forwarding entry points. */
-extern "C" int ra_engine_step(ra_engine* e, const ra_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
-                              size_t* n_msgs, ra_note* notes, size_t notes_cap, size_t* n_notes)
-{ return ra_emu_step((ra_emu*)e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
-extern "C" int ra_engine_get_cfg(ra_engine* e, ra_engine_cfg* out) { return ra_emu_get_cfg((ra_emu*)e, out); }
 
 /* ---- the record-plane codec on its own: one ABI record through st_rec_plane / ld_rec_plane ---------- */
 extern "C" int ra_emu_codec_roundtrip(const ra_event* in, ra_event* out, int* had_tail)
@@ -541,13 +533,10 @@ extern "C" int ra_emu_codec_roundtrip(const ra_event* in, ra_event* out, int* ha
     st_rec(out, ld_rec_plane(plane, 1, 0, row));
     return RA_OK;
 }
-extern "C" int ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
-                                   size_t* n_msgs, ra_note* notes, size_t notes_cap, size_t* n_notes)
-{ return ra_emu_step_host((ra_emu*)e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
 /* the split-phase calls with the two-slot contract of include/ra_engine.h: the emulation evaluates a call when it is
  * submitted and hands the result over at collect.  A call submitted behind a rejected one gets the same status, one
  * submitted behind a call whose outputs did not fit gets RA_E_PENDING; neither is evaluated. */
-static int submit_call(ra_emu* m, const void* ev, size_t n_ev, bool host32, ra_event* msgs, size_t msgs_cap,
+static int submit_call(ra_engine* m, const void* ev, size_t n_ev, bool host32, ra_event* msgs, size_t msgs_cap,
                        ra_note* notes, size_t notes_cap)
 {
     if (!m || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
@@ -564,10 +553,10 @@ static int submit_call(ra_emu* m, const void* ev, size_t n_ev, bool host32, ra_e
 }
 extern "C" int ra_engine_submit_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
                                      ra_note* notes, size_t notes_cap)
-{ return submit_call((ra_emu*)e, ev, n_ev, true, msgs, msgs_cap, notes, notes_cap); }
+{ return submit_call(e, ev, n_ev, true, msgs, msgs_cap, notes, notes_cap); }
 extern "C" int ra_engine_submit(ra_engine* e, const ra_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
                                 ra_note* notes, size_t notes_cap)
-{ return submit_call((ra_emu*)e, ev, n_ev, false, msgs, msgs_cap, notes, notes_cap); }
+{ return submit_call(e, ev, n_ev, false, msgs, msgs_cap, notes, notes_cap); }
 extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg* segs, size_t n_segs, ra_event* msgs,
                                           size_t msgs_cap, ra_note* notes, size_t notes_cap)
 {
@@ -583,28 +572,12 @@ extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg*
 }
 extern "C" int ra_engine_collect(ra_engine* e, size_t* n_msgs, size_t* n_notes)
 {
-    ra_emu* m = (ra_emu*)e;
-    if (!m || !m->sub_n) return RA_E_INVAL;                      // nothing submitted
-    const auto s = m->sub[0];
-    m->sub[0] = m->sub[1];
-    if (--m->sub_n == 0) m->sub_abort = 0;
-    if (s.rc == RA_E_CAPACITY && m->out_held) m->out_held = 0;   // the caller learns of the outputs waiting to be fetched
+    if (!e || !e->sub_n) return RA_E_INVAL;                      // nothing submitted
+    const auto s = e->sub[0];
+    e->sub[0] = e->sub[1];
+    if (--e->sub_n == 0) e->sub_abort = 0;
+    if (s.rc == RA_E_CAPACITY && e->out_held) e->out_held = 0;   // the caller learns of the outputs waiting to be fetched
     if (n_msgs) *n_msgs = s.nm;
     if (n_notes) *n_notes = s.nn;
     return s.rc;
 }
-
-/* ---- the rest of the ABI the dirty-NIF shim (ra_b200/csrc/ra_engine_nif.c) calls, so that it links against this
- * emulation on the CPU tier */
-extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out) { return ra_emu_create(cfg, (ra_emu**)out); }
-extern "C" void ra_engine_destroy(ra_engine* e) { ra_emu_destroy((ra_emu*)e); }
-extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
-{ return ra_emu_load_rows((ra_emu*)e, rows, n); }
-extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n) { return ra_emu_read_rows((ra_emu*)e, rows, n); }
-extern "C" int ra_engine_reset_empty(ra_engine* e) { return ra_emu_reset_empty((ra_emu*)e); }
-extern "C" int ra_engine_counters(ra_engine* e, ra_counters* out) { return ra_emu_counters((ra_emu*)e, out); }
-extern "C" int ra_engine_fetch_output(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                      ra_note* notes, size_t notes_cap, size_t* n_notes)
-{ return ra_emu_fetch_output((ra_emu*)e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
-extern "C" int ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes)
-{ return ra_emu_pending_output((ra_emu*)e, n_msgs, n_notes); }

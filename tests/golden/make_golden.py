@@ -103,12 +103,7 @@ FLOODS = [
 def rows_bytes_digest(b, chunk=65536) -> str:
     h = hashlib.sha256()
     for lo in range(0, b.n_rows, chunk):
-        hi = min(b.n_rows, lo + chunk)
-        arr = (abi.RaRowState * (hi - lo))()
-        for i in range(hi - lo):
-            arr[i].row = lo + i
-        b._check(b._fn("read_rows")(b._h, arr, hi - lo), "read_rows")
-        h.update(bytes(arr))
+        h.update(b"".join(bytes(r) for r in b.read_rows(range(lo, min(b.n_rows, lo + chunk)))))
     return h.hexdigest()
 
 

@@ -9,27 +9,59 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _declared():
+def _prototypes():
+    """{name: (returns void, number of parameters)} of every function include/ra_engine.h declares"""
     src = open(os.path.join(ROOT, "include", "ra_engine.h")).read()
-    return sorted(set(re.findall(r"\b(ra_engine_[a-z_]+)\s*\(", src)))
+    out = {}
+    for ret, name, params in re.findall(r"^([A-Za-z_][\w \t*]*?)\s*\b(ra_\w+)\s*\(([^;{]*?)\)\s*;", src, re.M | re.S):
+        params = params.strip()
+        out[name] = (ret.strip() == "void", 0 if params in ("", "void") else params.count(",") + 1)
+    return out
+
+
+def _table():
+    from ra_b200 import abi
+    return {**{"ra_engine_" + k: v for k, v in abi.SIGNATURES.items()},
+            **{"ra_" + k: v for k, v in abi.HOST_SIGNATURES.items()}}
 
 
 def test_header_symbols_exported():
     so = os.path.join(ROOT, "ra_b200", "csrc", "libra_engine.so")
     assert os.path.exists(so), "build the engine first: python -c 'import __graft_entry__ as g; g.build()'"
     lib = ctypes.CDLL(so)
-    names = _declared()
+    names = sorted(_prototypes())
     assert len(names) >= 10
     for n in names:
         assert hasattr(lib, n), n
-    from ra_b200 import engine
-    assert sorted(engine.EXPORTS) == names
-    src = open(os.path.join(ROOT, "include", "ra_engine.h")).read()
-    sim = sorted(set(re.findall(r"\b(ra_hostsim_[a-z_]+)\s*\(", src)))
-    assert sim == sorted(engine.HOSTSIM_EXPORTS)
-    for n in sim + engine.HOST_EXPORTS:
-        assert hasattr(lib, n), n
-    assert sorted(set(re.findall(r"\b(ra_wal_[a-z_]+|ra_notes16_[a-z_]+)\s*\(", src))) == sorted(engine.HOST_EXPORTS)
+    assert sorted(_table()) == names
+
+
+def test_signature_table_matches_header():
+    """Every entry of the signature table has the header prototype's parameter count, and agrees on void."""
+    protos = _prototypes()
+    for name, (restype, argtypes) in _table().items():
+        assert protos[name] == (restype is None, len(argtypes)), (name, protos[name])
+
+
+def test_binding_ignores_declarations_on_the_shared_library():
+    """Backend calls go through private function objects: what another caller declares on the library's own
+    attribute for a symbol does not change them."""
+    import emu_lib
+    from ra_b200 import abi
+
+    def run():
+        e = emu_lib.Emu(8, 3, route_on_device=True)
+        e.reset_empty()
+        msgs, notes = e.step_host([abi.ev_simple(e.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(8)])
+        return [m.key() for m in msgs], [n.key() for n in notes]
+    want = run()
+    assert want[1]
+    shared = emu_lib.lib().ra_engine_step_host
+    shared.argtypes = [ctypes.c_int]
+    try:
+        assert run() == want
+    finally:
+        shared.argtypes = None
 
 
 def test_record_sizes_match_header():

@@ -24,12 +24,11 @@ import test_emu_fuzz as fz
 import test_kernel_fuzz as kf
 from oracle_lib import Oracle
 from ra_b200 import abi
-from ra_b200.engine import Engine
+from ra_b200.engine import Engine, notes16_expand
 from ra_suite import make_backend
 
 HOST_TYPES = {abi.EV_WRITTEN, abi.EV_COMMAND, abi.EV_ELECTION_TIMEOUT, abi.EV_AWAIT_COND_TIMEOUT, abi.EV_PIPELINE_RPCS,
               abi.EV_TICK, abi.EV_CONSISTENT_QUERY}
-SZ = C.c_size_t
 
 
 def host_event(rng, st, m):
@@ -45,14 +44,6 @@ def _caps(b):
     return b.n_rows * abi.RA_MSG_CAP, b.n_rows * abi.RA_NOTE_CAP
 
 
-def _abi(b, name, *argtypes):
-    """an entry point by its include/ra_engine.h name (the emulation library exports the split-phase ones too)"""
-    f = getattr(b._lib, "ra_engine_" + name)
-    f.restype = C.c_int
-    f.argtypes = list(argtypes)
-    return f
-
-
 def _segments(rng, evs):
     """1..256 pieces cut at row boundaries (a row's events never straddle two), some of them empty"""
     bounds = [0] + [i for i in range(1, len(evs)) if evs[i].row != evs[i - 1].row] + [len(evs)]
@@ -61,32 +52,18 @@ def _segments(rng, evs):
     return [evs[a:b] for a, b in zip(edges, edges[1:])]
 
 
-class _Seg(C.Structure):
-    _fields_ = [("ev", C.c_void_p), ("n", SZ)]
-
-
-def _call(b, path, evs, rng=None, msgs_cap=None, notes_cap=None):
+def _call(b, path, evs, rng=None):
     """One batch through `path` with ample buffers -> (msgs, notes)."""
     mc, nc = _caps(b)
-    mc, nc = msgs_cap or mc, notes_cap or nc
     if path == "step":
         return b.step(evs, mc, nc)
-    msgs, notes = (abi.RaEvent * mc)(), (abi.RaNote * nc)()
-    nm, nn = SZ(0), SZ(0)
     if path == "step_host":
-        ev = (abi.RaHostEvent * max(len(evs), 1))(*[abi.RaHostEvent.of(e) for e in evs])
-        st = _abi(b, "step_host", C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.POINTER(SZ), C.c_void_p, SZ,
-                  C.POINTER(SZ))(b._h, ev, len(evs), msgs, mc, C.byref(nm), notes, nc, C.byref(nn))
-    else:
-        parts = _segments(rng, evs)
-        bufs = [(abi.RaHostEvent * max(1, len(p)))(*[abi.RaHostEvent.of(e) for e in p]) for p in parts]
-        segs = (_Seg * len(parts))(*[_Seg(C.addressof(x), len(p)) for x, p in zip(bufs, parts)])
-        st = _abi(b, "submit_host_segs", C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.c_void_p, SZ)(
-            b._h, segs, len(parts), msgs, mc, notes, nc)
-        assert st == abi.RA_OK
-        st = _abi(b, "collect", C.c_void_p, C.POINTER(SZ), C.POINTER(SZ))(b._h, C.byref(nm), C.byref(nn))
+        return b.step_host(evs, mc, nc)
+    st, ticket = b.submit_host_segs(_segments(rng, evs), mc, nc)
+    assert st == abi.RA_OK
+    st, _, _, msgs, notes = b.collect(ticket)
     assert st == abi.RA_OK, "%s: status %d" % (path, st)
-    return list(msgs[: nm.value]), list(notes[: nn.value])
+    return msgs, notes
 
 
 def _checker(o, m, bs, rnd, mode):
@@ -170,17 +147,6 @@ def encode16(notes, wal_c):
     return b"".join(units + ext), len(ext) // 2
 
 
-def _expand(units, n_notes, n_ext, last_c):
-    from ra_b200.engine import lib
-    f = lib().ra_notes16_expand
-    f.restype = SZ
-    f.argtypes = [C.c_void_p, SZ, SZ, C.c_void_p, C.c_void_p, SZ]
-    out = (abi.RaNote * max(n_notes, 1))()
-    buf = C.create_string_buffer(bytes(units), max(len(units), 1))
-    assert f(buf, n_notes, n_ext, last_c, out, max(n_notes, 1)) == n_notes
-    return list(out[:n_notes])
-
-
 FORMS = ("ext_slot", "range_256", "status_c", "above_2_32", "truncate", "query", "same_term")
 
 
@@ -213,7 +179,7 @@ class _RoundTrip(Oracle):
         _forms(notes, self.seen)
         units, n_ext = encode16(notes, self.wal_c)
         self.seen["same_term"] += sum(1 for k in range(len(notes)) if units[16 * k + 4] & abi.N16_SAME_TERM)
-        return msgs, _expand(units, len(notes), n_ext, self.last_c)
+        return msgs, notes16_expand(units, len(notes), n_ext, self.last_c)
 
 
 @pytest.mark.parametrize("mode", kf.MODES)
@@ -265,34 +231,16 @@ def test_compact_stream_unit_for_unit_engine(mode, monkeypatch):
 
 
 # ---- raw calls with counts on RA_E_CAPACITY -------------------------------------------------------------------------
-def _pending(b):
-    f = b._fn("pending_output")
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.POINTER(SZ), C.POINTER(SZ)]
-    nm, nn = SZ(0), SZ(0)
-    assert f(b._h, C.byref(nm), C.byref(nn)) == abi.RA_OK
-    return nm.value, nn.value
-
-
-def _last_ext(b):
-    f = b._lib.ra_engine_last_ext_count
-    f.restype = SZ
-    f.argtypes = [C.c_void_p]
-    return f(b._h)
-
-
 class _Out:
     """output buffers of one call: pageable ctypes arrays or pinned ra_engine_alloc_host memory; notes_cap counts
     32-byte notes or (compact) 16-byte units"""
 
     def __init__(self, b, msgs_cap, notes_cap, compact=False, pinned=False):
-        self.b, self.mc, self.nc, self.compact, self.pinned = b, msgs_cap, notes_cap, compact, pinned
+        self.mc, self.nc, self.compact, self.pinned = msgs_cap, notes_cap, compact, pinned
         nt = abi.RaNote16 if compact else abi.RaNote
         if pinned:
-            l = b._lib
-            l.ra_engine_alloc_host.restype = C.c_void_p
-            l.ra_engine_alloc_host.argtypes = [SZ]
-            self._p = [l.ra_engine_alloc_host(max(msgs_cap, 1) * 64), l.ra_engine_alloc_host(max(notes_cap, 1) * 32)]
+            self._api = b._api
+            self._p = [self._api.alloc_host(max(msgs_cap, 1) * 64), self._api.alloc_host(max(notes_cap, 1) * 32)]
             assert all(self._p)
             self.msgs = (abi.RaEvent * max(msgs_cap, 1)).from_address(self._p[0])
             self.notes = (nt * max(notes_cap, 1)).from_address(self._p[1])
@@ -301,46 +249,24 @@ class _Out:
 
     def free(self):
         if self.pinned:
-            f = self.b._lib.ra_engine_free_host
-            f.restype, f.argtypes = None, [C.c_void_p]
             for p in self._p:
-                f(p)
+                self._api.free_host(p)
             self.pinned = False
 
     def result(self, nm, nn, n_ext=0, last_c=None):
         msgs = [fz._copy(x) for x in self.msgs[:nm]]
         if not self.compact:
             return msgs, [abi.RaNote.from_buffer_copy(x) for x in self.notes[:nn]]
-        return msgs, _expand(bytes(self.notes)[: 16 * (nn + 2 * n_ext)], nn, n_ext, last_c)
+        return msgs, notes16_expand(bytes(self.notes)[: 16 * (nn + 2 * n_ext)], nn, n_ext, last_c)
 
     def units(self, nn, n_ext):
         return bytes(self.notes)[: 16 * (nn + 2 * n_ext)]
 
 
 def _submit(b, api, evs, out):
-    if api == "submit_host":
-        ev = (abi.RaHostEvent * max(len(evs), 1))(*[abi.RaHostEvent.of(e) for e in evs])
-    else:
-        ev = (abi.RaEvent * max(len(evs), 1))(*evs)
-    st = _abi(b, api, C.c_void_p, C.c_void_p, SZ, C.c_void_p, SZ, C.c_void_p, SZ)(
-        b._h, ev, len(evs), out.msgs, out.mc, out.notes, out.nc)
+    st, ticket = getattr(b, api)(evs, out.mc, out.nc, out=(out.msgs, out.notes))
     assert st == abi.RA_OK, "%s: status %d" % (api, st)
-    return ev                                                    # (kept alive until collected)
-
-
-def _collect(b):
-    nm, nn = SZ(0), SZ(0)
-    st = _abi(b, "collect", C.c_void_p, C.POINTER(SZ), C.POINTER(SZ))(b._h, C.byref(nm), C.byref(nn))
-    return st, nm.value, nn.value
-
-
-def _fetch(b, out):
-    nm, nn = SZ(0), SZ(0)
-    f = b._fn("fetch_output")
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_void_p, SZ, C.POINTER(SZ), C.c_void_p, SZ, C.POINTER(SZ)]
-    st = f(b._h, out.msgs, out.mc, C.byref(nm), out.notes, out.nc, C.byref(nn))
-    return st, nm.value, nn.value
+    return ticket                                                # (holds the batch until it is collected)
 
 
 def _batch(rng, o, m, G, draw, density):
@@ -396,7 +322,7 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
             what = "M=%d %s round %d batch %d" % (m, mode, rnd, k)
             n_ext = 0
             if compact:
-                n_ext = _last_ext(b)
+                n_ext = b.last_ext_count()
                 assert n_ext == wants[k][3], "%s: ra_engine_last_ext_count %d, the encoder %d" % (what, n_ext, wants[k][3])
                 assert out.units(nn, n_ext) == wants[k][2], "%s: compact units differ" % what
             got = out.result(nm, nn, n_ext, last_c)
@@ -406,8 +332,8 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
             out.free()
 
         def collect_oldest():
-            k, out, _ev = fly.pop(0)
-            st, nm, nn = _collect(b)
+            k, out, ticket = fly.pop(0)
+            st, nm, nn, _, _ = b.collect(ticket)
             cov["calls"] += 1
             msgs, notes = wants[k][1]
             what = "M=%d %s round %d batch %d" % (m, mode, rnd, k)
@@ -415,20 +341,20 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
                 cov["capacity"] += 1
                 assert (nm, nn) == (len(msgs), len(notes)), "%s: RA_E_CAPACITY reports %r, needed %r" % (
                     what, (nm, nn), (len(msgs), len(notes)))
-                assert _pending(b) == (len(msgs), len(notes)), "%s: pending_output %r" % (what, _pending(b))
+                assert b.pending_output() == (len(msgs), len(notes)), "%s: pending_output %r" % (what, b.pending_output())
                 behind = []
                 while fly:                                       # calls submitted behind it: not evaluated
-                    k2, out2, _ = fly.pop(0)
-                    st2, _, _ = _collect(b)
+                    k2, out2, ticket2 = fly.pop(0)
+                    st2 = b.collect(ticket2)[0]
                     assert st2 == abi.RA_E_PENDING, "%s: the call submitted behind it returned %d, not " \
                         "RA_E_PENDING" % (what, st2)
                     cov["pending"] += 1
                     out2.free()
                     behind.append(k2)
-                units = nn + 2 * _last_ext(b) if compact else nn
+                units = nn + 2 * b.last_ext_count() if compact else nn
                 out.free()
                 out = _Out(b, nm, units, compact, pinned)
-                st, nm2, nn2 = _fetch(b, out)
+                st, nm2, nn2, _, _ = b.fetch_output(out.mc, out.nc, out=(out.msgs, out.notes))
                 assert st == abi.RA_OK and (nm2, nn2) == (nm, nn), "%s: fetch of the reported size: %d %r" % (
                     what, st, (nm2, nn2))
                 finish(k, out, nm, nn)
@@ -449,7 +375,7 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
                 collect_oldest()
         while fly:
             collect_oldest()
-        assert kf._rows_bytes(b) == kf._rows_bytes(o), "M=%d %s round %d: rows differ" % (m, mode, rnd)
+        assert b.rows_bytes() == o.rows_bytes(), "M=%d %s round %d: rows differ" % (m, mode, rnd)
         assert b.counters() == o.counters()
     return cov
 

@@ -2,24 +2,12 @@
 instead of 32-byte notes on the device->host path.  The decoder must rebuild exactly the notes the plain format
 carries; in the steady-state flood every note is one unit."""
 import ctypes as C
-import os
 
 import pytest
 
 from ra_b200 import abi
+from ra_b200.engine import notes16_expand
 from ra_suite import *  # noqa: F401,F403
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _expand(units, n_notes, n_ext, last_c):
-    l = C.CDLL(os.path.join(ROOT, "ra_b200", "csrc", "libra_engine.so"))
-    f = l.ra_notes16_expand
-    f.restype = C.c_size_t
-    f.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]
-    out = (abi.RaNote * max(n_notes, 1))()
-    assert f(units, n_notes, n_ext, last_c, out, max(n_notes, 1)) == n_notes
-    return [(n.row, n.type, n.slot, n.aux, n.a, n.b, n.c) for n in out[:n_notes]]
 
 
 def test_expand_hand_made_units():
@@ -36,7 +24,7 @@ def test_expand_hand_made_units():
     ext[0], ext[1], ext[2], ext[3] = 10, 12, 7, 0            # {a, b}, {c, 0}
     ext[4], ext[5], ext[6], ext[7] = 99, 0x03000102, 6, 0
     last_c = (C.c_uint64 * 8)()
-    got = _expand(units, 4, 2, last_c)
+    got = [(n.row, n.type, n.slot, n.aux, n.a, n.b, n.c) for n in notes16_expand(units, 4, 2, last_c)]
     assert got == [(3, NOTE_WAL_APPEND, 0, 0, 10, 12, 7), (3, NOTE_WAL_APPEND, 0, 0, 13, 13, 7),
                    (3, NOTE_APPLY, 0, 4, 9, 12, 0), (5, NOTE_STATUS, 2, 3, 99, 0x03000102, 6)]
     assert last_c[3] == 7

@@ -47,18 +47,6 @@ def test_trace_parity_emu_small_pipeline_window():
     assert got == want
 
 
-def _rows_bytes(b, n_rows, chunk=65536):
-    out = []
-    for lo in range(0, n_rows, chunk):
-        hi = min(n_rows, lo + chunk)
-        arr = (abi.RaRowState * (hi - lo))()
-        for i in range(hi - lo):
-            arr[i].row = lo + i
-        b._check(b._fn("read_rows")(b._h, arr, hi - lo), "read_rows")
-        out.append(bytes(arr))
-    return b"".join(out)
-
-
 def _bootstrap(b):
     b.reset_empty()
     b.step([abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(b.n_groups)])
@@ -85,7 +73,7 @@ def test_flood_parity_emu(g, m, steps, cmds, permille):
         e.flood(part, cmds, permille, seed=42)
     assert e.counters() == o.counters()
     assert o.counters()["commits"] > 0
-    ro, re_ = _rows_bytes(o, o.n_rows), _rows_bytes(e, e.n_rows)
+    ro, re_ = o.rows_bytes(), e.rows_bytes()
     sz = C.sizeof(abi.RaRowState)
     first = next((i // sz for i in range(0, len(ro), sz) if ro[i:i + sz] != re_[i:i + sz]), -1)
     assert re_ == ro, "first differing row: %d" % first
@@ -126,7 +114,7 @@ def test_host_driven_flood_equals_device_flood_emu(threads, monkeypatch):
     """ra_hostsim_run (the product's host-side caller, every step through step() with host buffers)
     leaves exactly the rows the device-side flood leaves, and both equal the oracle -- the CPU twin
     of tests/test_parity_gpu.py::test_host_driven_flood_equals_device_flood."""
-    from emu_lib import EmuHostFlood
+    from ra_b200.engine import HostFlood
     monkeypatch.setenv("RA_HOSTSIM_THREADS", threads)
     g, m, steps = 1200, 5, 70
     a = Emu(g, m, route_on_device=True)
@@ -137,14 +125,14 @@ def test_host_driven_flood_equals_device_flood_emu(threads, monkeypatch):
     _bootstrap(o)
     o.flood(steps, 1, 10, seed=5, threads=2)
     b.reset_empty()
-    hf = EmuHostFlood(b)
+    hf = HostFlood(b)
     st = hf.run(steps, 1, 10, seed=5, bootstrap=True)
     assert st["h2d_bytes"] > 0 and st["d2h_bytes"] > 0 and st["engine_calls"] == steps + 1
     ca, cb, co = a.counters(), b.counters(), o.counters()
     assert ca == co
     for k in ("events", "commits", "applied", "msgs_out", "elections_won"):
         assert cb[k] == ca[k]
-    assert _rows_bytes(b, b.n_rows) == _rows_bytes(a, a.n_rows)
+    assert b.rows_bytes() == a.rows_bytes()
     hf.close()
 
 
@@ -190,10 +178,8 @@ def test_record_plane_codec_is_lossless():
     rec_decode): every field the logic reads comes back bit-identical for arbitrary records, the shapes
     the steady state relies on really are heads only, and stale bytes of the tile never leak."""
     import random
-    from emu_lib import lib
-    l = lib()
-    l.ra_emu_codec_roundtrip.restype = C.c_int
-    l.ra_emu_codec_roundtrip.argtypes = [C.POINTER(abi.RaEvent), C.POINTER(abi.RaEvent), C.POINTER(C.c_int)]
+    from emu_lib import extras
+    roundtrip = extras().codec_roundtrip
     rng = random.Random(7)
     big = [0, 1, 2, 5, 2**32 - 1, 2**32, 2**63, 2**64 - 1]
 
@@ -202,7 +188,7 @@ def test_record_plane_codec_is_lossless():
 
     def check(e, want_tail=None):
         out, tail = abi.RaEvent(), C.c_int(-1)
-        assert l.ra_emu_codec_roundtrip(C.byref(e), C.byref(out), C.byref(tail)) == 0
+        assert roundtrip(C.byref(e), C.byref(out), C.byref(tail)) == 0
         # row and seq are positional inside a plane (the reader knows them), _pad is scratch
         got = (out.type, out.from_slot, out.flags, out.n, out.n1, out.term, out.a, out.b, out.c, out.d, out.e)
         exp = (e.type, e.from_slot, e.flags, e.n, e.n1, e.term, e.a, e.b, e.c, e.d, e.e)

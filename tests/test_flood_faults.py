@@ -22,19 +22,6 @@ def _run(be, g, m, steps, cmds, permille, faults, seed=0xA05):
     return b
 
 
-def _rows(b):
-    import ctypes as C
-    out = []
-    for lo in range(0, b.n_rows, 65536):
-        hi = min(b.n_rows, lo + 65536)
-        arr = (abi.RaRowState * (hi - lo))()
-        for i in range(hi - lo):
-            arr[i].row = lo + i
-        b._check(b._fn("read_rows")(b._h, arr, hi - lo), "read_rows")
-        out.append(bytes(arr))
-    return b"".join(out)
-
-
 CASES = [
     ("emu", 200, 7, 300, 1, 0, FAULTS),
     ("emu", 300, 5, 200, 2, 10, (20, 50, 30, 16)),
@@ -57,4 +44,4 @@ def test_fault_flood_equals_oracle(be, g, m, steps, cmds, permille, faults):
         assert co["aer_replies_failed"] > 0                    # missing -> failure reply -> back-off
     if faults[2] and steps * g >= 30_000:
         assert co["elections_won"] > g                         # leaders changed
-    assert _rows(e) == _rows(o)
+    assert e.rows_bytes() == o.rows_bytes()

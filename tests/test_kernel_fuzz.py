@@ -24,8 +24,8 @@ from emu_lib import Emu
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_suite import make_backend
-from test_record_forms import HEAD, LONG, _rows_bytes
-from test_short_records import StatsEmu, plane_forms
+from test_record_forms import HEAD, LONG
+from test_short_records import plane_forms, stats_lib
 
 MEMBERS = [3, 4, 5, 7, 8]
 MODES = ["pure", "chased", "routed", "flood"]
@@ -47,7 +47,7 @@ def _kw(mode, note_cap=0):
 def _observe(b, m, out=None):
     msgs, notes = out if out is not None else ([], [])
     q = b.read_query_state(range(b.n_rows))
-    return dict(msgs=[x.key() for x in msgs], notes=[x.key() for x in notes], rows=_rows_bytes(b),
+    return dict(msgs=[x.key() for x in msgs], notes=[x.key() for x in notes], rows=b.rows_bytes(),
                 counters=b.counters(), query=[x.key(m) for x in q])
 
 
@@ -197,7 +197,7 @@ def test_kernel_fuzz_routed_twin():
     in the mailbox planes (no host event is ingested in them)."""
     G, m = 48, 5
     rng = random.Random(4321)
-    o, e = Oracle(G, m, **_kw("routed")), StatsEmu(G, m, **_kw("routed"))
+    o, e = Oracle(G, m, **_kw("routed")), Emu(G, m, library=stats_lib(), **_kw("routed"))
     heads = longs = cmds = 0
     for rnd in range(4):
         loads, qs, events = _fuzz_round(rng, o, m, G, rnd)
@@ -212,7 +212,7 @@ def test_kernel_fuzz_routed_twin():
         heads += forms[abi.EV_AER][HEAD]
         longs += forms[abi.EV_AER][LONG]
         cmds += forms[abi.EV_COMMAND][HEAD] + forms[abi.EV_COMMAND][LONG]
-        assert _rows_bytes(e) == _rows_bytes(o)
+        assert e.rows_bytes() == o.rows_bytes()
     assert heads > 0 and longs > 0, (heads, longs)
     assert cmds == 0                                           # (commands only come from the host)
 
@@ -308,7 +308,7 @@ def test_reloaded_fatal_row_gets_no_stale_mail(backend):
     for k, (w, x) in enumerate(zip(want, got)):
         assert x == w, "step %d differs" % k
     assert b.counters() == o.counters()
-    assert _rows_bytes(b) == _rows_bytes(o)
+    assert b.rows_bytes() == o.rows_bytes()
 
 
 def _flood_then_step(b):

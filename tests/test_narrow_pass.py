@@ -23,14 +23,6 @@ def _auto_mode(monkeypatch):
     monkeypatch.delenv("RA_STEP_WIDE", raising=False)
 
 
-def _rows_bytes(b):
-    arr = (abi.RaRowState * b.n_rows)()
-    for i in range(b.n_rows):
-        arr[i].row = i
-    b._check(b._fn("read_rows")(b._h, arr, b.n_rows), "read_rows")
-    return bytes(arr)
-
-
 def _keys(out):
     msgs, notes = out
     return [m.key() for m in msgs], [n.key() for n in notes]
@@ -59,7 +51,7 @@ def _flood_pair(o, e, base, term, steps, cmds, permille):
         e.flood(part, cmds, permille, seed=77)
     assert e.counters() == o.counters()
     assert o.counters()["commits"] > 0
-    ro, re_ = _rows_bytes(o), _rows_bytes(e)
+    ro, re_ = o.rows_bytes(), e.rows_bytes()
     sz = C.sizeof(abi.RaRowState)
     first = next((i // sz for i in range(0, len(ro), sz) if ro[i:i + sz] != re_[i:i + sz]), -1)
     assert re_ == ro, "first differing row: %d" % first
@@ -112,7 +104,7 @@ def test_narrow_and_wide_pass_agree_emu(monkeypatch):
         # a leaderless cluster answering pre-votes by hand is enough to run followers' fast paths
         log.append(_keys(e.step([abi.ev_pre_vote(e.row_of(g, 1), 0, 0, 1, 0, 0) for g in range(40)])))
         log.append(_keys(e.step([abi.ev_aer(e.row_of(g, 2), 0, 1, 0, 0, 0, [1, 1]) for g in range(40)])))
-        outs.append((log, _rows_bytes(e), Emu.narrow_stats()))
+        outs.append((log, e.rows_bytes(), Emu.narrow_stats()))
     assert outs[0][0] == outs[1][0] and outs[0][1] == outs[1][1]
     assert outs[0][2]["rows_narrow"] > 0 and outs[1][2]["rows_narrow"] == 0
 
@@ -128,7 +120,7 @@ def _wide_record_script(b, groups):
                             abi.ev_written(b.row_of(g, 1), big if g % 2 else 1, 2, 2),
                             abi.ev_aer(b.row_of(g, 1), 0, big if g % 2 else 1, 2, big if g % 2 else 1, 1, []))])))
     t.append(_keys(b.step([abi.ev_aer(b.row_of(g, 1), 0, big if g % 2 else 1, 2, big if g % 2 else 1, 2, []) for g in range(groups)])))
-    return t, _rows_bytes(b)
+    return t, b.rows_bytes()
 
 
 def test_record_with_a_wide_field_goes_to_the_general_path_emu():
@@ -223,7 +215,7 @@ def test_pipeline_limits_beyond_31_bits_emu(kw):
         b.step([abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(50)])
     o.flood(60, 3, 20, seed=5, threads=1)
     e.flood(60, 3, 20, seed=5)
-    assert e.counters() == o.counters() and _rows_bytes(e) == _rows_bytes(o) and o.counters()["commits"] > 0
+    assert e.counters() == o.counters() and e.rows_bytes() == o.rows_bytes() and o.counters()["commits"] > 0
     # and a lossy closed-loop trace (failure replies move next_index below match_index + 1: in_flight < 0)
     batches = trace_gen.generate(lambda gg, mm: Oracle(gg, mm, **kw), 8, 5, 200, 3, p_drop=0.08, p_cmd=0.9, max_cmd=9)
     assert trace_gen.replay(Emu(8, 5, **kw), batches) == trace_gen.replay(Oracle(8, 5, **kw), batches)

@@ -244,7 +244,7 @@ def o_step(o, evs):
 
 
 def same_state(eng, o, what):
-    got, want = eng.rows_bytes(), kf._rows_bytes(o)
+    got, want = eng.rows_bytes(), o.rows_bytes()
     assert isinstance(got, bytes), "%s: read_rows returned %r" % (what, got)
     if got != want:
         raise AssertionError("%s: rows differ from row %d" % (what, kf._first_row(want, got)))

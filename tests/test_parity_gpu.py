@@ -63,18 +63,6 @@ def test_trace_parity_small_pipeline_window():
     assert got == want and got_rows == want_rows and got_cnt == want_cnt
 
 
-def _rows_bytes(b, n_rows, chunk=65536):
-    out = []
-    for lo in range(0, n_rows, chunk):
-        hi = min(n_rows, lo + chunk)
-        arr = (abi.RaRowState * (hi - lo))()
-        for i in range(hi - lo):
-            arr[i].row = lo + i
-        b._check(b._fn("read_rows")(b._h, arr, hi - lo), "read_rows")
-        out.append(bytes(arr))
-    return b"".join(out)
-
-
 def _first_diff(a: bytes, b: bytes) -> int:
     sz = C.sizeof(abi.RaRowState)
     for i in range(0, len(a), sz):
@@ -112,7 +100,7 @@ def test_flood_parity(g, m, steps, cmds, permille):
     co, ce = o.counters(), e.counters()
     assert ce == co
     assert co["commits"] > 0
-    ro, re_ = _rows_bytes(o, o.n_rows), _rows_bytes(e, e.n_rows)
+    ro, re_ = o.rows_bytes(), e.rows_bytes()
     assert re_ == ro, "first differing row: %d" % _first_diff(ro, re_)
 
 
@@ -128,7 +116,7 @@ def test_flood_parity_full_size_and_properties():
         else:
             b.flood(steps, 1, 10, seed=9)
     assert e.counters() == o.counters()
-    ro, re_ = _rows_bytes(o, o.n_rows), _rows_bytes(e, e.n_rows)
+    ro, re_ = o.rows_bytes(), e.rows_bytes()
     assert re_ == ro, "first differing row: %d" % _first_diff(ro, re_)
     # properties on the engine's rows (sampled groups)
     rows = e.read_rows([e.row_of(gg, s) for gg in range(0, g, 997) for s in range(m)])
@@ -188,5 +176,5 @@ def test_host_driven_flood_equals_device_flood():
     assert ca == co
     for k in ("events", "commits", "applied", "msgs_out", "elections_won"):
         assert cb[k] == ca[k]
-    ra, rb = _rows_bytes(a, a.n_rows), _rows_bytes(b, b.n_rows)
+    ra, rb = a.rows_bytes(), b.rows_bytes()
     assert rb == ra, "first differing row: %d" % _first_diff(ra, rb)

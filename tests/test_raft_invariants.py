@@ -40,7 +40,6 @@ GPU, `engine` with RA_STEP_WIDE=0 and =1), and nothing asks it for expected valu
 from __future__ import annotations
 
 import bisect
-import ctypes as C
 import random
 
 import numpy as np
@@ -67,23 +66,12 @@ def _backend(name, g, m, monkeypatch, width=None, **kw):
 
 
 def read_all(b) -> np.ndarray:
-    arr = (abi.RaRowState * b.n_rows)()
-    for i in range(b.n_rows):
-        arr[i].row = i
-    b._check(b._fn("read_rows")(b._h, arr, b.n_rows), "read_rows")
-    return np.frombuffer(arr, dtype=ROW_DT).copy()
+    return np.frombuffer(b.rows_bytes(), dtype=ROW_DT).copy()
 
 
 def step(b, batch):
     """One ra_engine_step with room for every row's outputs -> (RPC records, notes)."""
-    n = len(batch)
-    ev = (abi.RaEvent * max(n, 1))(*batch)
-    mc = 1024 if b.cfg.route_on_device else b.n_rows * abi.RA_MSG_CAP
-    nc = b.n_rows * abi.RA_NOTE_CAP
-    msgs, notes = (abi.RaEvent * mc)(), (abi.RaNote * nc)()
-    nm, nn = C.c_size_t(0), C.c_size_t(0)
-    b._check(b._fn("step")(b._h, ev, n, msgs, mc, C.byref(nm), notes, nc, C.byref(nn)), "step")
-    return list(msgs[: nm.value]), list(notes[: nn.value])
+    return b.step(batch, 1024 if b.cfg.route_on_device else b.n_rows * abi.RA_MSG_CAP, b.n_rows * abi.RA_NOTE_CAP)
 
 
 # ---- logs as term runs ------------------------------------------------------------------------------------------

@@ -10,7 +10,7 @@ steps also every record and note.
 
 CPU tier: the host emulation (tests/emu) reads the bytes the kernel would not have fetched as poison and counts every
 record it decoded from them (Emu.underfetched), so a lost flag shows there.  Each case has a twin at reduced size on
-the plane-stats build (test_short_records.StatsEmu) that asserts the precondition: the targeted records really were
+the plane-stats build (test_short_records.stats_lib()) that asserts the precondition: the targeted records really were
 stored as heads (or long).  GPU tier: the same cases on the engine, with the 32-bit (RA_STEP_WIDE=0) and the 64-bit
 (RA_STEP_WIDE=1) hot kernel.
 """
@@ -20,13 +20,12 @@ from collections import defaultdict
 
 import pytest
 
-import test_short_records as short_records
 import trace_gen
 from emu_lib import Emu, EmuShards
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_suite import make_backend
-from test_short_records import StatsEmu, plane_forms
+from test_short_records import plane_forms, stats_lib
 
 BACKENDS = ["emu", pytest.param("engine", marks=pytest.mark.gpu)]
 WIDTHS = ["0", "1"]                       # RA_STEP_WIDE: the 32-bit hot kernel / the 64-bit one
@@ -39,13 +38,9 @@ def _poison_and_underfetch():
     """The emulation's cases alternate the two poison patterns (by pass, see _make) and must end without a record
     decoded from bytes the kernel did not fetch; every test starts with both libraries' counts at zero."""
     Emu.underfetched()
-    _twin_underfetched()
+    Emu.underfetched(library=stats_lib())
     yield
     Emu.set_fetch_poison(0)
-
-
-def _stats_call(name, *args):
-    return getattr(short_records._lib(), name)(*args)
 
 
 def _make(name, wide, monkeypatch, groups, members, **kw):
@@ -60,29 +55,9 @@ def _check_fetch(name):
         assert Emu.underfetched() == 0, "the hot path decoded a record from bytes its tile's fetch did not cover"
 
 
-def _twin_underfetched():
-    arr = (C.c_ulonglong * 1)()
-    _stats_call("ra_emu_fetch_stats", arr, 1)
-    return int(arr[0])
-
-
-def _twin_stalls():
-    arr = (C.c_ulonglong * 2)()
-    _stats_call("ra_emu_stall_stats", arr, 1)
-    return dict(stalls=arr[0], stalls_wk_hi=arr[1])
-
-
-def _rows_bytes(b):
-    arr = (abi.RaRowState * b.n_rows)()
-    for i in range(b.n_rows):
-        arr[i].row = i
-    b._check(b._fn("read_rows")(b._h, arr, b.n_rows), "read_rows")
-    return bytes(arr)
-
-
 def _same_rows(got, want):
     sz = C.sizeof(abi.RaRowState)
-    a, b = _rows_bytes(got), _rows_bytes(want)
+    a, b = got.rows_bytes(), want.rows_bytes()
     first = next((i // sz for i in range(0, len(a), sz) if a[i:i + sz] != b[i:i + sz]), -1)
     assert a == b, "first differing row: %d" % first
 
@@ -136,12 +111,12 @@ def test_flood_with_head_and_long_records(members, cmds, batch, faults, backend,
 
 @pytest.mark.parametrize("members,cmds,batch,faults", FLOODS, ids=FLOOD_IDS)
 def test_flood_with_head_and_long_records_twin(members, cmds, batch, faults):
-    e = StatsEmu(48, members, route_on_device=True, max_aer_batch=batch)
+    e = Emu(48, members, library=stats_lib(), route_on_device=True, max_aer_batch=batch)
     _bootstrap(e)
     plane_forms()
     e.flood(40, cmds, PERMILLE, SEED, faults)
     forms = plane_forms()
-    assert _twin_underfetched() == 0
+    assert Emu.underfetched(library=stats_lib()) == 0
     assert e.counters()["commits"] > 0
     if cmds < 256:
         assert all(h == 0 for _, h, _ in forms.values()), forms
@@ -185,9 +160,9 @@ def test_trace_with_long_batches(members, backend, wide, monkeypatch):
 @pytest.mark.parametrize("members", [3, 5, 7])
 def test_trace_with_long_batches_twin(members):
     plane_forms()
-    _replay_equal(StatsEmu(10, members, max_aer_batch=512), members)
+    _replay_equal(Emu(10, members, library=stats_lib(), max_aer_batch=512), members)
     forms = plane_forms()
-    assert _twin_underfetched() == 0
+    assert Emu.underfetched(library=stats_lib()) == 0
     assert forms[abi.EV_COMMAND][HEAD] > 0 and forms[abi.EV_AER][HEAD] > 0, forms
 
 
@@ -231,11 +206,11 @@ def test_scripted_step_mixes_every_form_in_a_tile(members, backend, wide, monkey
 
 
 def test_scripted_step_mixes_every_form_in_a_tile_twin():
-    e = StatsEmu(40, 5)
+    e = Emu(40, 5, library=stats_lib())
     plane_forms()
     _scripted(e)
     forms = plane_forms()
-    assert _twin_underfetched() == 0
+    assert Emu.underfetched(library=stats_lib()) == 0
     assert forms[abi.EV_COMMAND][SHORT] > 0 and forms[abi.EV_COMMAND][HEAD] > 0, forms[abi.EV_COMMAND]
     assert forms[abi.EV_AER][HEAD] > 0 and forms[abi.EV_AER][LONG] > 0, forms[abi.EV_AER]
     assert forms[abi.EV_AER_REPLY][HEAD] > 0 and forms[abi.EV_PRE_VOTE][LONG] > 0, forms
@@ -288,11 +263,11 @@ def test_step_host_long_commands_and_wide_written(backend, wide, monkeypatch):
 
 @pytest.mark.parametrize("wide_values", [False, True])
 def test_step_host_long_commands_and_wide_written_twin(wide_values):
-    e = StatsEmu(40, 5, route_on_device=True, max_aer_batch=512)
+    e = Emu(40, 5, library=stats_lib(), route_on_device=True, max_aer_batch=512)
     plane_forms()
     _host_loop(e, wide_values)
     forms = plane_forms()
-    assert _twin_underfetched() == 0
+    assert Emu.underfetched(library=stats_lib()) == 0
     assert forms[abi.EV_COMMAND][HEAD] > 0 and forms[abi.EV_AER][HEAD] > 0, forms
     if wide_values:
         assert forms[abi.EV_WRITTEN][HEAD] > 0 and forms[abi.EV_WRITTEN][SHORT] == 0, forms[abi.EV_WRITTEN]
@@ -386,11 +361,11 @@ def test_head_record_sent_before_a_stall(backend, wide, monkeypatch):
 
 
 def test_head_record_sent_before_a_stall_twin():
-    e = StatsEmu(64, 5, route_on_device=True, max_aer_batch=512)
-    _twin_stalls()
+    e = Emu(64, 5, library=stats_lib(), route_on_device=True, max_aer_batch=512)
+    Emu.stall_stats(library=stats_lib())
     plane_forms()
     _stall_crossing(e)
     forms = plane_forms()
-    assert _twin_underfetched() == 0
+    assert Emu.underfetched(library=stats_lib()) == 0
     assert forms[abi.EV_AER][HEAD] >= 4 * 64, forms[abi.EV_AER]
-    assert _twin_stalls()["stalls_wk_hi"] >= 64
+    assert Emu.stall_stats(library=stats_lib())["stalls_wk_hi"] >= 64

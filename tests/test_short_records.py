@@ -13,6 +13,7 @@ import tempfile
 
 import pytest
 
+from emu_lib import Emu
 from ra_b200 import abi
 
 SHORT, HEAD, LONG = 0, 1, 3          # what st_rec_plane reports: nothing but chunk 0 / chunks 0-1 / chunks 0-3
@@ -21,9 +22,9 @@ _SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu", "plane_st
 _lib_cache = []
 
 
-def _lib():
+def stats_lib():
     """tests/emu/plane_stats.cpp: the host emulation built with per-form store counters, compiled on first use into a
-    temporary directory (the tree is left as it is)."""
+    temporary directory (the tree is left as it is).  Emu(..., library=stats_lib()) runs on it."""
     if _lib_cache:
         return _lib_cache[0]
     d = tempfile.mkdtemp(prefix="ra_plane_stats_")
@@ -31,30 +32,20 @@ def _lib():
     so = os.path.join(d, "libra_plane_stats.so")
     subprocess.check_call([os.environ.get("CXX", "g++"), "-O1", "-std=c++17", "-fPIC", "-shared", "-Wl,-Bsymbolic",
                            "-Wl,--no-undefined", "-o", so, _SRC])
-    l = C.CDLL(so)
-    f = l.ra_emu_codec_roundtrip2
-    f.restype = C.c_int
-    f.argtypes = [C.POINTER(abi.RaEvent), C.c_int, C.POINTER(abi.RaEvent), C.POINTER(C.c_int),
-                  C.POINTER(abi.RaEvent), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    l.ra_emu_plane_forms.restype = None
-    l.ra_emu_plane_forms.argtypes = [C.POINTER(C.c_ulonglong), C.c_int]
-    l.ra_emu_flood_faults.restype = C.c_int
-    l.ra_emu_flood_faults.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64,
-                                      C.POINTER(abi.RaFloodFaults)]
-    _lib_cache.append(l)
-    return l
+    _lib_cache.append(C.CDLL(so))
+    return _lib_cache[0]
 
 
-class StatsEmu(abi.Backend):
-    """The emulation of the plane-stats build (same entry points as tests/emu_lib.Emu)."""
-    name = "emu_stats"
+_int_p = C.POINTER(C.c_int)
+EXTRAS = {                                     # ra_emu_<name> of the plane-stats build
+    "codec_roundtrip2": (C.c_int, [C.POINTER(abi.RaEvent), C.c_int, C.POINTER(abi.RaEvent), _int_p,
+                                   C.POINTER(abi.RaEvent), _int_p, _int_p]),
+    "plane_forms": (None, [C.POINTER(C.c_ulonglong), C.c_int]),
+}
 
-    def __init__(self, n_groups: int, n_members: int, **kw):
-        super().__init__(_lib(), "ra_emu", n_groups, n_members, **kw)
 
-    def flood(self, n_steps, cmds, permille, seed, faults=None):
-        ff = C.byref(abi.RaFloodFaults(*faults)) if faults else None
-        self._check(_lib().ra_emu_flood_faults(self._h, n_steps, cmds, permille, seed, ff), "flood_faults")
+def _stats():
+    return abi.bind(stats_lib(), "ra_emu", EXTRAS)
 
 
 def _fields(e):
@@ -63,12 +54,11 @@ def _fields(e):
 
 def roundtrip(e, want_form):
     """Store e through both passes over tiles full of stale bytes; every field the logic reads comes back."""
-    l = _lib()
     fits_narrow = max(e.term, e.a, e.b, e.c, e.d, e.e) < NARROW_LIMIT
     for fill in (0x00, 0xA5, 0xFF):
         ow, on = abi.RaEvent(), abi.RaEvent()
         form, fits, form_n = C.c_int(-1), C.c_int(-1), C.c_int(-1)
-        assert l.ra_emu_codec_roundtrip2(C.byref(e), fill, C.byref(ow), C.byref(form), C.byref(on), C.byref(fits),
+        assert _stats().codec_roundtrip2(C.byref(e), fill, C.byref(ow), C.byref(form), C.byref(on), C.byref(fits),
                                          C.byref(form_n)) == 0
         assert form.value == want_form, (fill, _fields(e))
         assert _fields(ow) == _fields(e) and ow._pad == 0, (fill, _fields(ow), _fields(e))
@@ -129,7 +119,6 @@ def test_random_records_roundtrip():
     import random
     rng = random.Random(11)
     vals = [0, 1, 2**30 - 1, 2**30, 2**32 - 1, 2**32, 2**64 - 1]
-    l = _lib()
     for _ in range(5000):
         t = rng.choice(vals + [rng.getrandbits(rng.choice([8, 31, 33]))])
         e = abi.RaEvent(row=rng.randrange(1 << 20), type=rng.randrange(20), from_slot=rng.choice([0, 5, 7, 8, 15, 255]),
@@ -138,7 +127,7 @@ def test_random_records_roundtrip():
                         c=rng.choice([t, 0, rng.choice(vals)]), d=rng.choice([0, 1, t]), e=rng.choice([0, 0, 5]))
         ow, on = abi.RaEvent(), abi.RaEvent()
         form, fits, form_n = C.c_int(-1), C.c_int(-1), C.c_int(-1)
-        assert l.ra_emu_codec_roundtrip2(C.byref(e), rng.randrange(256), C.byref(ow), C.byref(form), C.byref(on),
+        assert _stats().codec_roundtrip2(C.byref(e), rng.randrange(256), C.byref(ow), C.byref(form), C.byref(on),
                                          C.byref(fits), C.byref(form_n)) == 0
         assert _fields(ow) == _fields(e)
         if fits.value:
@@ -149,7 +138,7 @@ def test_random_records_roundtrip():
 
 def plane_forms():
     arr = (C.c_ulonglong * 64)()
-    _lib().ra_emu_plane_forms(arr, 1)
+    _stats().plane_forms(arr, 1)
     return {t: (arr[4 * t + SHORT], arr[4 * t + HEAD], arr[4 * t + LONG]) for t in range(16)}
 
 
@@ -163,7 +152,7 @@ SHAPES = [
 
 @pytest.mark.parametrize("shape", SHAPES, ids=["config3", "config4", "config5"])
 def test_steady_state_records_are_written_short(shape):
-    e = StatsEmu(shape["groups"], shape["members"], route_on_device=True)
+    e = Emu(shape["groups"], shape["members"], library=stats_lib(), route_on_device=True)
     e.reset_empty()
     e.step([abi.ev_simple(e.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(shape["groups"])])
     e.flood(20, shape["cmds"], shape["permille"], seed=0xA03, faults=shape["faults"])

@@ -134,27 +134,13 @@ def test_rejected_batch_takes_the_one_behind_it_along():
 @pytest.mark.gpu
 def test_submit_host_segs_equals_one_batch():
     """a batch of host events handed over in pieces (one per producer thread) = the same batch in one array"""
-    import ctypes as C
-    from ra_b200.engine import lib
     a = _cluster("engine", 64, 3, route_on_device=True)
     b = _cluster("engine", 64, 3, route_on_device=True)
     evs = [ev_simple(a.row_of(g, 0), EV_ELECTION_TIMEOUT) for g in range(64)]
     want = a.step_host(evs)
-
-    class Seg(C.Structure):
-        _fields_ = [("ev", C.c_void_p), ("n", C.c_size_t)]
-    parts = [evs[0:10], [], evs[10:40], evs[40:64]]
-    bufs = [(abi.RaHostEvent * max(1, len(p)))(*[abi.RaHostEvent.of(e) for e in p]) for p in parts]
-    segs = (Seg * len(parts))(*[Seg(C.addressof(bf), len(p)) for bf, p in zip(bufs, parts)])
-    l = lib()
-    f = l.ra_engine_submit_host_segs
-    f.restype = C.c_int
-    sz = C.c_size_t
-    f.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.c_void_p, sz]
-    msgs = (abi.RaEvent * 1024)()
-    notes = (abi.RaNote * 4096)()
-    assert f(b._h, segs, len(parts), msgs, 1024, notes, 4096) == RA_OK
-    st, nm, nn, gm, gn = b.collect((None, msgs, notes))
+    st, ticket = b.submit_host_segs([evs[0:10], [], evs[10:40], evs[40:64]], 1024, 4096)
+    assert st == RA_OK
+    st, nm, nn, gm, gn = b.collect(ticket)
     assert st == RA_OK
     assert [x.key() for x in gm] == [x.key() for x in want[0]] and [x.key() for x in gn] == [x.key() for x in want[1]]
     assert [r.key() for r in a.read_rows(range(a.n_rows))] == [r.key() for r in b.read_rows(range(b.n_rows))]

@@ -9,39 +9,23 @@ import pytest
 from emu_lib import Emu
 from oracle_lib import Oracle
 from ra_b200 import abi
+from ra_b200.engine import host
 from ra_suite import base_state, make_backend
-
-
-class Writer(C.Structure):
-    _fields_ = [("row", C.c_uint32), ("n_ranges", C.c_uint32), ("term", C.c_uint64), ("ranges", C.POINTER(C.c_uint64))]
-
-
-class Resume(C.Structure):
-    _fields_ = [("writer", C.c_uint32), ("range", C.c_uint32)]
-
-
-def _lib():
-    from ra_b200.engine import lib              # host-only entry point: no device needed
-    l = lib()
-    l.ra_wal_batch_to_events.restype = C.c_size_t
-    l.ra_wal_batch_to_events.argtypes = [C.POINTER(Writer), C.c_size_t, C.c_uint32, C.POINTER(abi.RaEvent), C.c_size_t,
-                                         C.POINTER(Resume)]
-    return l
 
 
 def batch_events(writers, max_per_row=abi.RA_LOCAL_CAP, cap=1024):
     """writers: [(row, term, [(from, to), ...])] -> list of per-step event lists"""
     keep = []
-    arr = (Writer * len(writers))()
+    arr = (abi.RaWalWriter * len(writers))()
     for i, (row, term, ranges) in enumerate(writers):
         flat = (C.c_uint64 * (2 * len(ranges)))(*[x for r in ranges for x in r])
         keep.append(flat)
-        arr[i] = Writer(row, len(ranges), term, flat)
-    res = Resume(0, 0)
+        arr[i] = abi.RaWalWriter(row, len(ranges), term, flat)
+    res = abi.RaWalResume(0, 0)
     out = (abi.RaEvent * cap)()
     steps = []
     while res.writer < len(writers):
-        n = _lib().ra_wal_batch_to_events(arr, len(writers), max_per_row, out, cap, C.byref(res))
+        n = host().wal_batch_to_events(arr, len(writers), max_per_row, out, cap, C.byref(res))   # no device needed
         assert n > 0
         steps.append([abi.RaEvent.from_buffer_copy(bytes(out[i])) for i in range(n)])
     return steps

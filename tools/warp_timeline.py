@@ -12,7 +12,6 @@ The raw per-warp records go to OUT/timeline_<step>.npy and the summary to OUT/ti
     python tools/warp_timeline.py [--so PATH] [--out DIR] [--groups N] [--members M] [--steps K]
 """
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -44,11 +43,7 @@ if not os.path.exists(a.so):
 os.environ["RA_ENGINE_SO"] = a.so
 sys.path.insert(0, ROOT)
 from ra_b200 import abi                      # noqa: E402
-from ra_b200.engine import Engine, lib       # noqa: E402
-
-f = lib().ra_engine_warp_timeline
-f.restype = C.c_int
-f.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+from ra_b200.engine import Engine            # noqa: E402
 
 e = Engine(a.groups, a.members, route_on_device=True)
 e.reset_empty()
@@ -118,12 +113,10 @@ def summarise(t):
 
 steps = []
 for k in range(a.steps):
-    f(e._h, None, 0)
+    e.call("warp_timeline", None, 0)
     e.flood(1, a.cmds, a.permille, seed=0xA00)
     buf = np.zeros(n_warps * TL_WORDS, dtype=np.uint64)
-    rc = f(e._h, buf.ctypes.data, buf.size)
-    if rc != 0:
-        raise SystemExit("ra_engine_warp_timeline failed: %d" % rc)
+    e.call("warp_timeline", buf.ctypes.data, buf.size)
     t = buf.reshape(n_warps, TL_WORDS)
     np.save(os.path.join(a.out, "timeline_%d.npy" % k), t)
     steps.append(summarise(t))
