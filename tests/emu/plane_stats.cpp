@@ -2,7 +2,7 @@
  *
  * The host emulation (ra_emu.cpp, compiled into this one translation unit unchanged) built with RA_PLANE_STATS:
  * every record the device logic stores into a record plane is counted by type and form, and the record-plane codec
- * is exposed through both index widths.  tests/test_short_records.py compiles this file on its own (g++, into a
+ * is exposed through both index widths.  tests/emu_lib.py (stats_lib) compiles this file on its own (g++, into a
  * temporary directory) and loads it next to the regular emulation library; both export the same names, so it
  * is linked -Bsymbolic and loaded RTLD_LOCAL (ctypes' default).
  */

@@ -5,9 +5,13 @@ it is never imported by the product package and is not a fallback for it.
 """
 from __future__ import annotations
 
+import atexit
 import ctypes as C
 import os
+import shutil
 import subprocess
+import tempfile
+from collections import namedtuple
 
 from ra_b200 import abi
 
@@ -30,13 +34,35 @@ def lib() -> C.CDLL:
     return _lib
 
 
+_stats_lib = None
+
+
+def stats_lib() -> C.CDLL:
+    """tests/emu/plane_stats.cpp: the host emulation built with per-form store counters, compiled on first use into a
+    temporary directory (the tree is left as it is).  Emu(..., library=stats_lib()) runs on it."""
+    global _stats_lib
+    if _stats_lib is None:
+        d = tempfile.mkdtemp(prefix="ra_plane_stats_")
+        atexit.register(shutil.rmtree, d, True)
+        so = os.path.join(d, "libra_plane_stats.so")
+        subprocess.check_call([os.environ.get("CXX", "g++"), "-O1", "-std=c++17", "-fPIC", "-shared", "-Wl,-Bsymbolic",
+                               "-Wl,--no-undefined", "-o", so, os.path.join(_DIR, "plane_stats.cpp")])
+        _stats_lib = C.CDLL(so)
+    return _stats_lib
+
+
 _ull_p = C.POINTER(C.c_ulonglong)
+_int_p = C.POINTER(C.c_int)
 EXTRAS = {                                     # ra_emu_<name>: the emulation's own calls, process-wide per library
     "narrow_stats": (None, [_ull_p, C.c_int]),
     "stall_stats": (None, [_ull_p, C.c_int]),
     "fetch_stats": (None, [_ull_p, C.c_int]),
     "set_fetch_poison": (None, [C.c_int]),
     "codec_roundtrip": (C.c_int, [C.POINTER(abi.RaEvent), C.POINTER(abi.RaEvent), C.POINTER(C.c_int)]),
+    # the plane-stats build only
+    "codec_roundtrip2": (C.c_int, [C.POINTER(abi.RaEvent), C.c_int, C.POINTER(abi.RaEvent), _int_p,
+                                   C.POINTER(abi.RaEvent), _int_p, _int_p]),
+    "plane_forms": (None, [_ull_p, C.c_int]),
 }
 
 
@@ -45,9 +71,20 @@ def extras(library: C.CDLL | None = None) -> abi.Binding:
     return abi.bind(library or lib(), "ra_emu", EXTRAS)
 
 
+SHORT, HEAD, LONG = 0, 1, 3          # what st_rec_plane reports: nothing but chunk 0 / chunks 0-1 / chunks 0-3
+Forms = namedtuple("Forms", "short head long")
+
+
+def plane_forms() -> dict:
+    """Records the plane-stats build stored into a record plane since the last call, by type: {type: Forms}."""
+    arr = (C.c_ulonglong * 64)()
+    extras(stats_lib()).plane_forms(arr, 1)
+    return {t: Forms(arr[4 * t + SHORT], arr[4 * t + HEAD], arr[4 * t + LONG]) for t in range(16)}
+
+
 class Emu(abi.Backend):
-    """The emulation in `library` (default: tests/emu/libra_emu.so; tests/test_short_records.py builds a plane-stats
-    one).  The stats calls are process-wide: they read the counters of `library`, by default of libra_emu.so."""
+    """The emulation in `library` (default: tests/emu/libra_emu.so; stats_lib() builds a plane-stats one).  The stats
+    calls are process-wide: they read the counters of `library`, by default of libra_emu.so."""
     name = "emu"
 
     def __init__(self, n_groups: int, n_members: int, library: C.CDLL | None = None, **kw):

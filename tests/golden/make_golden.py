@@ -30,6 +30,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import trace_gen                      # noqa: E402
 from oracle_lib import Oracle          # noqa: E402
 from ra_b200 import abi                # noqa: E402
+from ra_suite import clone             # noqa: E402
 
 TRACES = {
     # name: (groups, members, steps, seed, simulator knobs, engine config)
@@ -60,7 +61,7 @@ def rows_digest(backend) -> str:
 def replay_digests(backend, batches):
     out = []
     for batch in batches:
-        msgs, notes = backend.step([trace_gen.copy_ev(e) for e in batch])
+        msgs, notes = backend.step([clone(e) for e in batch])
         out.append(digest_outputs(msgs, notes))
     return out, rows_digest(backend), backend.counters()
 

@@ -29,10 +29,40 @@ def make_backend(name: str, n_groups: int, n_members: int, **kw):
     raise ValueError(name)
 
 
-def clone(s: abi.RaRowState) -> abi.RaRowState:
-    d = abi.RaRowState()
-    C.memmove(C.byref(d), C.byref(s), C.sizeof(s))
+def clone(x):
+    """a copy of any ctypes record (row state, event, note, query state)"""
+    d = type(x)()
+    C.memmove(C.byref(d), C.byref(x), C.sizeof(x))
     return d
+
+
+def closed_loop(b, steps: int, step_fn) -> List[Tuple[list, list]]:
+    """A host-routed closed loop from an election timeout on every group's slot-0 member: every RPC record goes back
+    in as an event of the next step, WAL_APPEND notes as written events, leaders get a command every third step.
+    step_fn(events) -> (msgs, notes) steps b; returns the keys of every step's outputs."""
+    evs = [abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(b.n_groups)]
+    out = []
+    for t in range(steps):
+        evs.sort(key=lambda e: e.row)
+        # at most RA_LOCAL_CAP per row
+        take, rest, cnt = [], [], {}
+        for e in evs:
+            c = cnt.get(e.row, 0)
+            (take if c < 4 else rest).append(e)
+            cnt[e.row] = c + 1
+        msgs, notes = step_fn(take)
+        out.append(([m.key() for m in msgs], [n.key() for n in notes]))
+        evs = rest
+        for m in msgs:
+            evs.append(clone(m))
+            evs[-1].seq = 0
+        for n in notes:
+            if n.type == abi.NOTE_WAL_APPEND:
+                evs.append(abi.ev_written(n.row, n.c, n.a, n.b))
+        if t % 3 == 0:
+            rows = b.read_rows(range(b.n_rows))
+            evs += [abi.ev_command(r.row, 1) for r in rows if r.role == abi.LEADER]
+    return out
 
 
 def empty_state(n_servers: int, me: int) -> abi.RaRowState:

@@ -1,7 +1,7 @@
 """Differential fuzz of the engine's host call paths: the ways a real caller (INTEGRATION.md, ra_engine_nif.c,
 ra_hostsim) hands batches over and takes outputs back, each against the oracle with ample buffers in the plain
-format.  States and events come from the generator of tests/test_emu_fuzz.py (rich = True) through the rounds of
-tests/test_kernel_fuzz.py: RPC records and notes in order, every row as raw ra_row_state bytes, counters and query
+format.  States and events come from the generator of tests/fuzz_lib.py (rich = True) through the rounds of the
+kernel fuzz: RPC records and notes in order, every row as raw ra_row_state bytes, counters and query
 state are compared.
 
 - host-event batches, each sent three ways: ra_engine_step_host (32-byte records), ra_engine_submit_host_segs split
@@ -20,28 +20,12 @@ import struct
 
 import pytest
 
-import test_emu_fuzz as fz
-import test_kernel_fuzz as kf
+from fuzz_lib import (HOST_TYPES, MEMBERS, MODES, batch, fuzz_round, fuzz_rounds, host_event, kw, rich_event,
+                      same_keys, widths)
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_b200.engine import Engine, notes16_expand
-from ra_suite import make_backend
-
-HOST_TYPES = {abi.EV_WRITTEN, abi.EV_COMMAND, abi.EV_ELECTION_TIMEOUT, abi.EV_AWAIT_COND_TIMEOUT, abi.EV_PIPELINE_RPCS,
-              abi.EV_TICK, abi.EV_CONSISTENT_QUERY}
-
-
-def host_event(rng, st, m):
-    """The rich generator, redrawn until it gives a host-origin kind (written, cmd, cmd_long, etmo, ctmo, tick,
-    pipe with EVF_INFO, cq)."""
-    while True:
-        e = fz.random_event(rng, st, m, rich=True)
-        if e.type in HOST_TYPES:
-            return e
-
-
-def _caps(b):
-    return b.n_rows * abi.RA_MSG_CAP, b.n_rows * abi.RA_NOTE_CAP
+from ra_suite import clone, make_backend
 
 
 def _segments(rng, evs):
@@ -52,27 +36,28 @@ def _segments(rng, evs):
     return [evs[a:b] for a, b in zip(edges, edges[1:])]
 
 
-def _call(b, path, evs, rng=None):
-    """One batch through `path` with ample buffers -> (msgs, notes)."""
-    mc, nc = _caps(b)
-    if path == "step":
-        return b.step(evs, mc, nc)
-    if path == "step_host":
-        return b.step_host(evs, mc, nc)
-    st, ticket = b.submit_host_segs(_segments(rng, evs), mc, nc)
-    assert st == abi.RA_OK
-    st, _, _, msgs, notes = b.collect(ticket)
-    assert st == abi.RA_OK, "%s: status %d" % (path, st)
-    return msgs, notes
+class _Path:
+    """A backend whose step() hands the batch over through one call path with ample buffers: ra_engine_step_host,
+    ra_engine_submit_host_segs with pieces cut by rng, or ra_engine_step."""
 
+    def __init__(self, b, path, rng):
+        self.b, self.path, self.rng = b, path, rng
 
-def _checker(o, m, bs, rnd, mode):
-    def check(what, outs, evs):
-        want = kf._observe(o, m, out=outs[0])
-        for (w, p, b), out in zip(bs, outs[1:]):
-            kf._compare(want, kf._observe(b, m, out=out), "M=%d %s round %d RA_STEP_WIDE=%s %s: %s"
-                        % (m, mode, rnd, w, p, what), evs, o)
-    return check
+    def __getattr__(self, name):
+        return getattr(self.b, name)
+
+    def step(self, evs):
+        b = self.b
+        mc, nc = b.n_rows * abi.RA_MSG_CAP, b.n_rows * abi.RA_NOTE_CAP
+        if self.path == "step":
+            return b.step(evs, mc, nc)
+        if self.path == "step_host":
+            return b.step_host(evs, mc, nc)
+        st, ticket = b.submit_host_segs(_segments(self.rng, evs), mc, nc)
+        assert st == abi.RA_OK
+        st, _, _, msgs, notes = b.collect(ticket)
+        assert st == abi.RA_OK, "%s: status %d" % (self.path, st)
+        return msgs, notes
 
 
 # ---- 1. host-event batches, three ways ------------------------------------------------------------------------------
@@ -81,46 +66,30 @@ HOST_MODES = ["routed", "flood"]
 
 
 def _host_fuzz(backend, mode, m, G, rounds, seed, monkeypatch):
-    rng, srng = random.Random(seed), random.Random(seed + 1)
-    o = Oracle(G, m, **kf._kw(mode))
+    srng = random.Random(seed + 1)
+    o = Oracle(G, m, **kw(mode))
     bs = []
-    for w in kf.WIDTHS:
-        monkeypatch.setenv("RA_STEP_WIDE", w)
-        bs += [(w, p, make_backend(backend, G, m, **kf._kw(mode))) for p in PATHS]
-    n_long = 0
-    for rnd in range(rounds):
-        loads, qs, events = kf._fuzz_round(rng, o, m, G, rnd, draw=host_event)
-        assert all(e.type in HOST_TYPES for e in events)
-        n_long += sum(1 for e in events if e.type == abi.EV_COMMAND and e.n >= 256)
-        for x in [o] + [b for *_, b in bs]:
-            x.load_rows(loads)
-            x.load_query_state(qs)
-        check = _checker(o, m, bs, rnd, mode)
+    for w in widths(monkeypatch):
+        bs += [("RA_STEP_WIDE=%s %s" % (w, p), _Path(make_backend(backend, G, m, **kw(mode)), p, srng)) for p in PATHS]
+    drawn = []
 
-        def step_all(evs):
-            return [o.step([fz._copy(e) for e in evs])] + [_call(b, p, [fz._copy(e) for e in evs], srng)
-                                                          for _, p, b in bs]
-        for k, evs in enumerate([events] + ([[], []] if mode == "routed" else [])):
-            check("step %d" % k, step_all(evs), evs)
-        if mode == "flood":
-            faults = kf.FAULTS if rnd % 2 else None
-            o.flood(4, kf.FLOOD_CMDS, kf.PERMILLE, seed=seed + rnd, threads=4, faults=faults)
-            for *_, b in bs:
-                b.flood(4, kf.FLOOD_CMDS, kf.PERMILLE, seed=seed + rnd, faults=faults)
-            check("the step after the flood", step_all([]), [])
-    assert n_long > 0                                            # commands of 256 and 1000 entries: n above 8 bits
-    return o
+    def draw(rng, st, members):
+        drawn.append(host_event(rng, st, members))
+        return drawn[-1]
+    fuzz_rounds(o, bs, mode, rounds, seed, draw=draw)
+    assert all(e.type in HOST_TYPES for e in drawn)
+    assert any(e.type == abi.EV_COMMAND and e.n >= 256 for e in drawn)   # commands of 256 and 1000 entries: n > 8 bits
 
 
 @pytest.mark.parametrize("mode", HOST_MODES)
-@pytest.mark.parametrize("m", kf.MEMBERS)
+@pytest.mark.parametrize("m", MEMBERS)
 def test_host_batches_three_ways_emu(m, mode, monkeypatch):
     _host_fuzz("emu", mode, m, 48, 4, 8000 + 10 * m + HOST_MODES.index(mode), monkeypatch)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", HOST_MODES)
-@pytest.mark.parametrize("m", kf.MEMBERS)
+@pytest.mark.parametrize("m", MEMBERS)
 def test_host_batches_three_ways_engine(m, mode, monkeypatch):
     _host_fuzz("engine", mode, m, 1200 if m <= 5 else 1024, 2, 8500 + 10 * m + HOST_MODES.index(mode), monkeypatch)
 
@@ -182,15 +151,15 @@ class _RoundTrip(Oracle):
         return msgs, notes16_expand(units, len(notes), n_ext, self.last_c)
 
 
-@pytest.mark.parametrize("mode", kf.MODES)
+@pytest.mark.parametrize("mode", MODES)
 def test_notes16_expand_on_fuzz_notes(mode):
     """every note the fuzz produces, through the reference encoder and the host decoder, comes back unchanged"""
     seen = dict.fromkeys(FORMS, 0)
     for m in (3, 5, 8):
-        _, bs, _ = kf._fuzz(lambda w, G, m, **kw: _RoundTrip(G, m, **kw), mode, m, 48, 4, 9000 + 10 * m)
-        for _, b in bs:
-            for k, v in b.seen.items():
-                seen[k] += v
+        b = _RoundTrip(48, m, **kw(mode))
+        fuzz_rounds(Oracle(48, m, **kw(mode)), [("notes16 round trip", b)], mode, 4, 9000 + 10 * m)
+        for k, v in b.seen.items():
+            seen[k] += v
     missing = [k for k in FORMS if not seen[k] and not (k == "query" and mode == "flood")]
     assert not missing, (missing, seen)
 
@@ -221,12 +190,10 @@ class _CompactEngine(Engine):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", kf.MODES)
+@pytest.mark.parametrize("mode", MODES)
 def test_compact_stream_unit_for_unit_engine(mode, monkeypatch):
-    def make(w, G, m, **kw):
-        monkeypatch.setenv("RA_STEP_WIDE", w)
-        return _CompactEngine(G, m, **kw)
-    _, bs, _ = kf._fuzz(make, mode, 5, 1200, 3, 9500 + kf.MODES.index(mode))
+    bs = [("RA_STEP_WIDE=" + w, _CompactEngine(1200, 5, **kw(mode))) for w in widths(monkeypatch)]
+    fuzz_rounds(Oracle(1200, 5, **kw(mode)), bs, mode, 3, 9500 + MODES.index(mode))
     assert all(b.ext > 0 for _, b in bs)
 
 
@@ -254,7 +221,7 @@ class _Out:
             self.pinned = False
 
     def result(self, nm, nn, n_ext=0, last_c=None):
-        msgs = [fz._copy(x) for x in self.msgs[:nm]]
+        msgs = [clone(x) for x in self.msgs[:nm]]
         if not self.compact:
             return msgs, [abi.RaNote.from_buffer_copy(x) for x in self.notes[:nn]]
         return msgs, notes16_expand(bytes(self.notes)[: 16 * (nn + 2 * n_ext)], nn, n_ext, last_c)
@@ -269,29 +236,16 @@ def _submit(b, api, evs, out):
     return ticket                                                # (holds the batch until it is collected)
 
 
-def _batch(rng, o, m, G, draw, density):
-    """a batch drawn from the oracle's current state (no reload: calls may be in flight)"""
-    evs = []
-    for st in o.read_rows(range(G * m)):
-        if rng.random() < density:
-            evs += [draw(rng, st, m) for _ in range(rng.randint(1, abi.RA_LOCAL_CAP))]
-    return evs
-
-
-def _rich(rng, st, m):
-    return fz.random_event(rng, st, m, rich=True)
-
-
 # ---- 2 + 3. two calls in flight; tight output buffers, one and two calls deep ---------------------------------------
 def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compact=False, pinned=False):
     """rounds of `steps` batches; every batch goes in while `depth - 1` calls are still in flight.  tight: each call's
     buffers hold 0 .. all of what it needs; a call answered RA_E_CAPACITY is fetched with exactly the reported size,
     and a call submitted behind it must come back RA_E_PENDING and is submitted again."""
-    draw = host_event if api == "submit_host" else _rich
+    draw = host_event if api == "submit_host" else rich_event
     wal_c, last_c = {}, ((C.c_uint64 * (G * m))() if compact else None)
     cov = dict(capacity=0, pending=0, calls=0)
     for rnd in range(rounds):
-        loads, qs, _ = kf._fuzz_round(rng, o, m, G, rnd, draw=draw)
+        loads, qs, _ = fuzz_round(rng, o, rnd, draw)
         for x in (o, b):
             x.load_rows(loads)
             x.load_query_state(qs)
@@ -325,10 +279,9 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
                 n_ext = b.last_ext_count()
                 assert n_ext == wants[k][3], "%s: ra_engine_last_ext_count %d, the encoder %d" % (what, n_ext, wants[k][3])
                 assert out.units(nn, n_ext) == wants[k][2], "%s: compact units differ" % what
-            got = out.result(nm, nn, n_ext, last_c)
-            outputs = lambda ms, ns: dict(msgs=[x.key() for x in ms], notes=[x.key() for x in ns], rows=b"",
-                                          counters=0, query=0)
-            kf._compare(outputs(msgs, notes), outputs(*got), what, wants[k][0], o)
+            got_msgs, got_notes = out.result(nm, nn, n_ext, last_c)
+            same_keys([x.key() for x in msgs], [x.key() for x in got_msgs], what, "msgs")
+            same_keys([x.key() for x in notes], [x.key() for x in got_notes], what, "notes")
             out.free()
 
         def collect_oldest():
@@ -365,9 +318,9 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
                 finish(k, out, nm, nn)
 
         for t in range(steps):
-            evs = _batch(rng, o, m, G, draw, rng.choice([0.02, 0.3, 1.0]))
+            evs = batch(rng, o, draw, rng.choice([0.02, 0.3, 1.0]))
             wal_c_at.append(dict(wal_c))
-            want = o.step([fz._copy(e) for e in evs], G * m * abi.RA_MSG_CAP, G * m * abi.RA_NOTE_CAP)
+            want = o.step([clone(e) for e in evs], G * m * abi.RA_MSG_CAP, G * m * abi.RA_NOTE_CAP)
             encode16(want[1], wal_c)                             # the per-row memory the engine keeps
             wants.append([evs, want, None, 0])
             submit(t)
@@ -386,7 +339,7 @@ def _chain(b, o, m, G, mode, api, rng, rounds, steps, depth, tight=False, compac
 def test_two_calls_in_flight_engine(api, pinned):
     G, m = 1200, 5
     rng = random.Random(9700 + 2 * (api == "submit_host") + pinned)
-    o, b = Oracle(G, m, **kf._kw("chased")), Engine(G, m, **kf._kw("chased"))
+    o, b = Oracle(G, m, **kw("chased")), Engine(G, m, **kw("chased"))
     cov = _chain(b, o, m, G, "chased", api, rng, rounds=2, steps=8, depth=2, pinned=pinned)
     assert cov["calls"] == 16
 
@@ -404,7 +357,7 @@ def test_tight_output_buffers(backend, fmt, depth, mode):
     fetch needs, and a call in flight behind it must change nothing"""
     G, m = (48, 5) if backend == "emu" else (1200, 5)
     rng = random.Random(9800 + 10 * depth + (fmt == "compact") + 100 * (mode == "routed"))
-    o, b = Oracle(G, m, **kf._kw(mode)), make_backend(backend, G, m, **kf._kw(mode))
+    o, b = Oracle(G, m, **kw(mode)), make_backend(backend, G, m, **kw(mode))
     if fmt == "compact":
         b.set_note_format(True)
     api = "submit" if backend == "engine" else "submit_host"      # (tests/test_nif_shim.py takes the emulation's submit)

@@ -39,7 +39,6 @@ def _cluster(groups=48, members=3):
 
 @pytest.mark.gpu
 def test_compact_stream_carries_the_same_notes():
-    from test_split_phase import _drive
     ref = _cluster()
     cp = _cluster()
     cp.set_note_format(True)
@@ -49,8 +48,8 @@ def test_compact_stream_carries_the_same_notes():
         msgs, notes, units, n_ext = cp.step_compact(evs)
         stats["notes"] += len(notes); stats["ext"] += n_ext; stats["units"] += len(units)
         return msgs, notes
-    want = _drive(ref, 30, lambda evs: ref.step(evs))
-    got = _drive(cp, 30, compact_step)
+    want = closed_loop(ref, 30, lambda evs: ref.step(evs))
+    got = closed_loop(cp, 30, compact_step)
     assert got == want
     assert [r.key() for r in cp.read_rows(range(cp.n_rows))] == [r.key() for r in ref.read_rows(range(ref.n_rows))]
     assert stats["notes"] > 500 and stats["ext"] < stats["notes"] // 3     # most notes are one unit

@@ -1,14 +1,15 @@
 """`-m "not gpu"`: host logic that needs no GPU -- trace generator determinism, the oracle's
 transport contract, and the N>1 sharding / reduction path of bench.py over gloo (world_size 2)."""
 import os
-import socket
 import subprocess
 import sys
 import textwrap
 
 import trace_gen
+from fuzz_lib import bootstrap, free_port
 from oracle_lib import Oracle
 from ra_b200 import abi
+from ra_suite import clone
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -38,8 +39,7 @@ def test_oracle_flood_thread_count_does_not_change_results():
     res = []
     for threads in (1, 3, 8):
         o = Oracle(300, 5, route_on_device=True)
-        o.reset_empty()
-        o.step([abi.ev_simple(o.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(300)])
+        bootstrap(o)
         o.flood(60, 1, 20, seed=4, threads=threads)
         res.append((o.counters(), [r.key() for r in o.read_rows(range(o.n_rows))]))
     assert res[0] == res[1] == res[2]
@@ -48,8 +48,7 @@ def test_oracle_flood_thread_count_does_not_change_results():
 
 def test_flood_commits_every_step_in_steady_state():
     o = Oracle(50, 5, route_on_device=True)
-    o.reset_empty()
-    o.step([abi.ev_simple(o.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(50)])
+    bootstrap(o)
     o.flood(40, 1, 0, seed=1)
     c0 = o.counters()["commits"]
     o.flood(100, 1, 0, seed=1)
@@ -67,19 +66,11 @@ def test_unrouted_and_routed_steps_agree_when_the_host_routes():
     b.step(boot)
     for _ in range(12):
         # deliver: order by destination row, then sender slot, then send order (contract item 7)
-        nxt = sorted((trace_gen.copy_ev(x) for x in msgs), key=lambda e: (e.row, e.from_slot, e.seq))
+        nxt = sorted((clone(x) for x in msgs), key=lambda e: (e.row, e.from_slot, e.seq))
         msgs, _ = a.step(nxt)
         b.step([])
     assert [r.key() for r in a.read_rows(range(a.n_rows))] == [r.key() for r in b.read_rows(range(b.n_rows))]
     assert any(r.role == abi.LEADER for r in a.read_rows(range(a.n_rows)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def test_group_sharding_over_gloo_world_size_2(tmp_path):
@@ -108,7 +99,7 @@ def test_group_sharding_over_gloo_world_size_2(tmp_path):
     """ % (ROOT, ROOT)))
     env = dict(os.environ, MASTER_ADDR="127.0.0.1")
     out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
-                          "--master-addr", "127.0.0.1", "--master-port", str(_free_port()), str(script)],
+                          "--master-addr", "127.0.0.1", "--master-port", str(free_port()), str(script)],
                          capture_output=True, text=True, env=env, timeout=300)
     assert out.returncode == 0, out.stderr[-2000:]
     import json
@@ -117,8 +108,7 @@ def test_group_sharding_over_gloo_world_size_2(tmp_path):
     assert r["ms"] == 20.0
     # the other rank's shard, recomputed here
     o = Oracle(200, 5, route_on_device=True)
-    o.reset_empty()
-    o.step([abi.ev_simple(o.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(200)])
+    bootstrap(o)
     o.flood(50, 1, 10, seed=101)
     assert r["commits"] == r["mine"] + o.counters()["commits"]
 

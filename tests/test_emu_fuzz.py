@@ -9,152 +9,10 @@ import random
 import pytest
 
 from emu_lib import Emu
+from fuzz_lib import (ROLES, compare, fuzz_around_the_narrow_limit, observe, random_event, random_query,
+                      random_state)
 from oracle_lib import Oracle
-from ra_b200 import abi
-
-ROLES = [abi.FOLLOWER, abi.CANDIDATE, abi.PRE_VOTE, abi.LEADER, abi.AWAIT_CONDITION]
-
-
-def random_state(rng: random.Random, row: int, n_groups: int, m: int, role: int, rich: bool = False) -> abi.RaRowState:
-    """rich = False draws exactly what the cases of this file always drew (their seeds stay meaningful); rich = True
-    (tests/test_kernel_fuzz.py) adds up to 8 term runs, the pending-pipeline flag, machine versions, promotable /
-    non-voter / unknown membership and all five peer statuses."""
-    s = abi.empty_row(row, n_groups, m)
-    me = s.self_slot
-    term = rng.randint(1, 12 if rich else 6)
-    # log: maybe a snapshot, then 0..4 (rich: 0..8) runs of non-decreasing terms <= term
-    has_snap = rng.random() < 0.3
-    snap_idx = rng.randint(1, 6) if has_snap else 0
-    snap_term = rng.randint(1, term) if has_snap else 0
-    entries = []
-    idx = snap_idx + 1 if has_snap else 0
-    t = snap_term if has_snap else 0
-    n_runs = rng.randint(0 if has_snap else 1, abi.RA_MAX_RUNS if rich else 4)
-    for _ in range(n_runs):
-        t = rng.randint(t, term) if entries or has_snap else (0 if rng.random() < 0.6 else rng.randint(0, term))
-        for _ in range(rng.randint(1, 4)):
-            entries.append((idx, t))
-            idx += 1
-        if t >= term:
-            break
-    abi.set_log(s, entries, snapshot=(snap_idx, snap_term) if has_snap else None)
-    last = s.last_index
-    lo = snap_idx if has_snap else 0
-
-    def term_at(i):
-        for (j, tt) in entries:
-            if j == i:
-                return tt
-        return snap_term if (has_snap and i == snap_idx) else None
-
-    lw = rng.randint(lo, last)
-    s.last_written_index, s.last_written_term = lw, term_at(lw) or 0
-    s.commit_index = rng.randint(lo, last + (2 if role != abi.LEADER and rng.random() < 0.2 else 0))
-    s.last_applied = rng.randint(lo, min(s.commit_index, last))
-    s.current_term = max(term, s.last_term)
-    s.role = role
-    s.voted_for = rng.choice([abi.RA_NO_SLOT] + list(range(m)))
-    s.leader_slot = me if role == abi.LEADER else rng.choice([abi.RA_NO_SLOT] + [p for p in range(m) if p != me])
-    s.votes = rng.randint(0, m // 2) if role in (abi.CANDIDATE, abi.PRE_VOTE) else 0
-    s.membership = abi.VOTER if rng.random() < 0.9 else (
-        rng.choice([abi.PROMOTABLE, abi.NON_VOTER, abi.UNKNOWN]) if rich else abi.PROMOTABLE)
-    s.pre_vote_token = rng.randint(1, 3)
-    s.token_counter = s.pre_vote_token + rng.randint(0, 2)
-    for p in range(m):
-        pe = s.peers[p]
-        pe.voter = 1 if (p == me and s.membership == abi.VOTER) or (p != me and rng.random() < 0.9) else 0
-        pe.next_index = rng.randint(max(1, lo), last + 1)
-        pe.match_index = rng.randint(0, pe.next_index - 1)
-        pe.commit_index_sent = rng.randint(0, s.commit_index)
-        pe.status = abi.PEER_NORMAL if rng.random() < 0.9 else rng.choice(
-            [abi.PEER_SENDING_SNAPSHOT, abi.PEER_SNAPSHOT_BACKOFF, abi.PEER_SUSPENDED, abi.PEER_DISCONNECTED] if rich else
-            [abi.PEER_SENDING_SNAPSHOT, abi.PEER_SUSPENDED, abi.PEER_DISCONNECTED])
-    if role == abi.AWAIT_CONDITION:
-        s.condition = 1                                  # follower catch-up (the condition on this path)
-        s.flags |= 2
-        s.cond_reply_term = s.current_term
-        s.cond_reply_next_index = last + 1
-        s.cond_reply_last_index = lw
-        s.cond_reply_last_term = s.last_written_term
-    if rich:
-        if rng.random() < 0.15:
-            s.flags |= 1                                 # a pipeline pass deferred from the step before
-        if rng.random() < 0.3:
-            s.machine_version, s.effective_machine_version = rng.randint(0, 3), rng.randint(0, 3)
-    return s
-
-
-def random_event(rng: random.Random, s: abi.RaRowState, m: int, rich: bool = False) -> abi.RaEvent:
-    """rich = True adds AppendEntries of 255, 256 and 300 entries (one or two term runs), replies from unknown slots
-    (9, 14, m) and commands of 256 and 1000 entries: records stored as 32-byte heads or 64-byte long records."""
-    row, me, term, last = s.row, s.self_slot, s.current_term, s.last_index
-    other = rng.choice([p for p in range(m) if p != me] or [me])
-    t = max(0, term + rng.choice([-1, 0, 0, 0, 1]))
-    near = lambda x: max(0, x + rng.choice([-2, -1, 0, 0, 0, 1, 2]))
-    kinds = ["aer", "aer", "reply", "reply", "rv", "rvres", "pv", "pvres", "written", "cmd",
-             "etmo", "ctmo", "tick", "pipe", "hb", "hbr", "cq"]
-    kind = rng.choice(kinds + ["aer_long", "reply_unknown", "cmd_long"] if rich else kinds)
-    if kind == "aer_long":
-        prev = near(last)
-        pt = rng.randint(0, t)
-        n = rng.choice([255, 256, 300])
-        t2 = rng.randint(pt, max(pt, t))
-        k = rng.choice([n, rng.randint(1, n - 1)])          # one term run, or two split at k
-        terms = [pt] * k + [t2] * (n - k)
-        return abi.ev_aer(row, other, t, prev, pt, near(s.commit_index), terms)
-    if kind == "reply_unknown":
-        return abi.ev_aer_reply(row, rng.choice([9, 14, m]), t, rng.random() < 0.7, near(last + 1), near(last),
-                                rng.randint(0, t))
-    if kind == "cmd_long":
-        return abi.ev_command(row, rng.choice([256, 1000]))
-    if kind == "hb":
-        return abi.ev_heartbeat_rpc(row, other, t, rng.randint(0, 4))
-    if kind == "hbr":
-        return abi.ev_heartbeat_reply(row, rng.choice([other, other, 7]), t, rng.randint(0, 4))
-    if kind == "cq":
-        return abi.ev_consistent_query(row)
-    if kind == "aer":
-        prev = near(last)
-        pt = rng.randint(0, t)
-        n = rng.choice([0, 0, 1, 2, 3])
-        terms = sorted(rng.randint(pt, max(pt, t)) for _ in range(n))
-        if len(set(terms)) > 2:
-            terms = [terms[0]] * (n - 1) + [terms[-1]]
-        return abi.ev_aer(row, other, t, prev, pt, near(s.commit_index), terms)
-    if kind == "reply":
-        li = near(last)
-        return abi.ev_aer_reply(row, other, t, rng.random() < 0.7, near(last + 1), li, rng.randint(0, t))
-    if kind == "rv":
-        return abi.ev_request_vote(row, other, t, near(last), rng.randint(0, t))
-    if kind == "rvres":
-        return abi.ev_request_vote_result(row, t, rng.random() < 0.7, voter=other)
-    if kind == "pv":
-        return abi.ev_pre_vote(row, other, t, rng.randint(1, 5), near(last), rng.randint(0, t),
-                               machine_version=rng.choice([0, 0, 1]))
-    if kind == "pvres":
-        return abi.ev_pre_vote_result(row, t, rng.choice([s.pre_vote_token, s.pre_vote_token + 1]),
-                                      rng.random() < 0.7, voter=other)
-    if kind == "written":
-        a = near(s.last_written_index + 1)
-        return abi.ev_written(row, rng.randint(max(0, term - 1), term), a, a + rng.randint(0, 3))
-    if kind == "cmd":
-        return abi.ev_command(row, rng.randint(1, 4))
-    if kind == "etmo":
-        return abi.ev_simple(row, abi.EV_ELECTION_TIMEOUT)
-    if kind == "ctmo":
-        return abi.ev_simple(row, abi.EV_AWAIT_COND_TIMEOUT)
-    if kind == "tick":
-        return abi.ev_simple(row, abi.EV_TICK)
-    e = abi.ev_simple(row, abi.EV_PIPELINE_RPCS)
-    e.flags = abi.EVF_INFO
-    return e
-
-
-def _copy(e: abi.RaEvent) -> abi.RaEvent:
-    import ctypes as C
-    d = abi.RaEvent()
-    C.memmove(C.byref(d), C.byref(e), C.sizeof(e))
-    return d
+from ra_suite import clone
 
 
 @pytest.mark.parametrize("m", [3, 5, 7])
@@ -173,118 +31,17 @@ def test_fuzz_state_event_pairs(m, pure):
             # up to two events for the row, adjacent in the batch (contract item 1)
             for _ in range(rng.choice([1, 1, 2])):
                 events.append(random_event(rng, st, m))
-        rows = [s.row for s in states]
-        qs = []
-        for st in states:                                   # consistent-query indexes of the row and its peers
-            q = abi.RaQueryState(row=st.row, query_index=rng.randint(0, 4), agreed_index=rng.randint(0, 2))
-            for p in range(m):
-                q.peer_query_index[p] = rng.randint(0, 4)
-            qs.append(q)
+        qs = [random_query(rng, st.row, m) for st in states]
         outs = []
         for b in (o, e):
             b.load_rows(states)
             b.load_query_state(qs)
-            msgs, notes = b.step([_copy(x) for x in events])
-            outs.append(([x.key() for x in msgs], [x.key() for x in notes],
-                         [r.key() for r in b.read_rows(rows)], b.counters(),
-                         [q.key(m) for q in b.read_query_state(rows)]))
-        w, x = outs
-        if w != x:
-            # narrow it down to the first row that differs, for the message
-            for i, (a, c) in enumerate(zip(w[2], x[2])):
-                if a != c:
-                    raise AssertionError("round %d row %d (role %d): rows differ\n oracle %r\n emu    %r\n events %r"
-                                         % (rnd, rows[i], states[i].role, a, c,
-                                            [(ev.type, ev.from_slot, ev.term, ev.a, ev.b, ev.c, ev.d, ev.e, ev.n, ev.n1)
-                                             for ev in events if ev.row == rows[i]]))
-            assert w[0] == x[0], "round %d: RPC records differ" % rnd
-            assert w[1] == x[1], "round %d: notes differ" % rnd
-            assert w[3] == x[3], "round %d: counters differ" % rnd
-            assert w[4] == x[4], "round %d: query state differs" % rnd
+            outs.append(observe(b, m, b.step([clone(x) for x in events])))
+        compare(outs[0], outs[1], "round %d" % rnd, events, o)
 
 
 # ---- the same corners, moved to where the hot kernel's 32-bit pass ends (tests/test_narrow_pass.py) ----------------
-LIM = 1 << 30
-OFFSETS = [(0, 0), (LIM - 9, 0), (0, LIM - 4), (LIM - 9, LIM - 4), (LIM + 5, 3), ((1 << 31) - 9, (1 << 31) - 4),
-           ((1 << 32) - 9, (1 << 32) - 4), ((1 << 40) + 1, 1 << 35)]
-
-
-def _shift_state(s: abi.RaRowState, di: int, dt: int, m: int) -> None:
-    for f in ("commit_index", "last_applied", "first_index", "last_index", "last_written_index", "snapshot_index",
-              "cond_reply_next_index", "cond_reply_last_index"):
-        setattr(s, f, getattr(s, f) + di)
-    for f in ("current_term", "last_term", "last_written_term", "snapshot_term", "cond_reply_term", "cond_reply_last_term"):
-        setattr(s, f, getattr(s, f) + dt)
-    for k in range(s.n_runs):
-        s.run_start[k] += di
-        s.run_term[k] += dt
-    for p in range(m):
-        s.peers[p].next_index += di
-        s.peers[p].match_index += di
-        s.peers[p].commit_index_sent += di
-
-
-def _shift_event(e: abi.RaEvent, di: int, dt: int) -> None:
-    t = e.type
-    if t == abi.EV_AER:
-        e.term += dt; e.a += di; e.b += dt; e.c += di; e.d += dt; e.e += dt
-    elif t == abi.EV_AER_REPLY:
-        e.term += dt; e.a += di; e.b += di; e.c += dt
-    elif t == abi.EV_REQUEST_VOTE or t == abi.EV_PRE_VOTE:
-        e.term += dt; e.a += di; e.b += dt
-    elif t in (abi.EV_REQUEST_VOTE_RES, abi.EV_PRE_VOTE_RES, abi.EV_HEARTBEAT_RPC, abi.EV_HEARTBEAT_REPLY):
-        e.term += dt
-    elif t == abi.EV_WRITTEN:
-        e.term += dt; e.a += di; e.b += di
-
-
 @pytest.mark.parametrize("pure", [True, False])
 def test_fuzz_state_event_pairs_around_the_narrow_limit(pure, monkeypatch):
     monkeypatch.delenv("RA_STEP_WIDE", raising=False)        # (the test asserts which pass ran)
-    _fuzz_around_the_narrow_limit(pure)
-
-
-def _fuzz_around_the_narrow_limit(pure, backend=Emu, G=64):
-    """Every row of a batch sits at its own distance from 2^30 / 2^31 / 2^32 (state and events moved together, and --
-    one time in five -- the events moved but not the state, or the other way round: records that do not fit handed to
-    rows that do).  M = 5: the emulated step kernel takes the 32-bit pass wherever it may.  backend: Emu, or the
-    engine (tests/test_kernel_fuzz.py) with G groups."""
-    m = 5
-    rng = random.Random(777 + (1 if pure else 0))
-    o, e = Oracle(G, m, pure=pure), backend(G, m, pure=pure)
-    Emu.narrow_stats()
-    for rnd in range(40):
-        states, events = [], []
-        for g in range(G):
-            slot = rng.randrange(m)
-            st = random_state(rng, slot * G + g, G, m, rng.choice(ROLES))
-            evs = [random_event(rng, st, m) for _ in range(rng.choice([1, 1, 2]))]
-            di, dt = rng.choice(OFFSETS)
-            mode = rng.random()
-            if mode < 0.9:
-                _shift_state(st, di, dt, m)
-            if mode > 0.1:
-                for ev in evs:
-                    _shift_event(ev, di, dt)
-            states.append(st)
-            events.extend(evs)
-        rows = [s.row for s in states]
-        outs = []
-        for b in (o, e):
-            b.load_rows(states)
-            msgs, notes = b.step([_copy(x) for x in events])
-            outs.append(([x.key() for x in msgs], [x.key() for x in notes], [r.key() for r in b.read_rows(rows)], b.counters()))
-        w, x = outs
-        if w != x:
-            for i, (a, c) in enumerate(zip(w[2], x[2])):
-                if a != c:
-                    raise AssertionError("round %d row %d (role %d): rows differ\n oracle %r\n emu    %r\n events %r"
-                                         % (rnd, rows[i], states[i].role, a, c,
-                                            [(ev.type, ev.from_slot, ev.term, ev.a, ev.b, ev.c, ev.d, ev.e, ev.n, ev.n1)
-                                             for ev in events if ev.row == rows[i]]))
-            assert w[0] == x[0], "round %d: RPC records differ" % rnd
-            assert w[1] == x[1], "round %d: notes differ" % rnd
-            assert w[3] == x[3], "round %d: counters differ" % rnd
-    if backend is Emu:
-        st = Emu.narrow_stats()
-        assert st["rows_narrow"] > 0 and st["rows_wide"] > 0 and st["records_refused"] > 0
+    fuzz_around_the_narrow_limit(pure)

@@ -11,6 +11,7 @@ import pytest
 
 import trace_gen
 from emu_lib import Emu
+from fuzz_lib import bootstrap, first_row
 from oracle_lib import Oracle
 from ra_b200 import abi
 
@@ -47,11 +48,6 @@ def test_trace_parity_emu_small_pipeline_window():
     assert got == want
 
 
-def _bootstrap(b):
-    b.reset_empty()
-    b.step([abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(b.n_groups)])
-
-
 FLOODS = [
     (64, 3, 60, 1, 0),
     (1000, 5, 80, 1, 0),
@@ -67,23 +63,21 @@ def test_flood_parity_emu(g, m, steps, cmds, permille):
     o = Oracle(g, m, route_on_device=True)
     e = Emu(g, m, route_on_device=True)
     for b in (o, e):
-        _bootstrap(b)
+        bootstrap(b)
     for part in (steps // 3, steps - steps // 3):
         o.flood(part, cmds, permille, seed=42, threads=2)
         e.flood(part, cmds, permille, seed=42)
     assert e.counters() == o.counters()
     assert o.counters()["commits"] > 0
     ro, re_ = o.rows_bytes(), e.rows_bytes()
-    sz = C.sizeof(abi.RaRowState)
-    first = next((i // sz for i in range(0, len(ro), sz) if ro[i:i + sz] != re_[i:i + sz]), -1)
-    assert re_ == ro, "first differing row: %d" % first
+    assert re_ == ro, "first differing row: %d" % first_row(ro, re_)
 
 
 def test_emu_fast_paths_carry_the_steady_state():
     """The stall histogram of the emulated step kernel: in a clean flood well under 1 % of the events
     leave the fast paths once leaders are elected (what keeps raft_general_kernel at ~3 % of a step)."""
     e = Emu(500, 5, route_on_device=True)
-    _bootstrap(e)
+    bootstrap(e)
     e.flood(30, 1, 0, seed=3)
     h0, ev0 = sum(e.stall_histogram().values()), e.counters()["events"]
     e.flood(50, 1, 0, seed=3)
@@ -120,9 +114,9 @@ def test_host_driven_flood_equals_device_flood_emu(threads, monkeypatch):
     a = Emu(g, m, route_on_device=True)
     b = Emu(g, m, route_on_device=True)
     o = Oracle(g, m, route_on_device=True)
-    _bootstrap(a)
+    bootstrap(a)
     a.flood(steps, 1, 10, seed=5)
-    _bootstrap(o)
+    bootstrap(o)
     o.flood(steps, 1, 10, seed=5, threads=2)
     b.reset_empty()
     hf = HostFlood(b)
@@ -157,8 +151,7 @@ def test_sharded_emu_equals_unsharded_oracle(n, m, gl, steps, permille, cmds):
     fl.run(steps, cmds, permille, seed=77)
     g = n * gl
     o = Oracle(g, m, route_on_device=True)
-    o.reset_empty()
-    o.step([abi.ev_simple(o.row_of(i, 0), abi.EV_ELECTION_TIMEOUT) for i in range(g)])
+    bootstrap(o)
     o.flood(steps, cmds, permille, seed=77, threads=2)
     want = {r.row: r.key()[1:] for r in o.read_rows(range(o.n_rows))}
     seen = 0

@@ -6,7 +6,7 @@ erlang/src/ra_engine_nif.erl; records travel as binaries of the ABI structs, as 
 The shim creates its engines with a zeroed ra_engine_cfg (not routed, not pure, default AER batch, pipeline count and
 note budget), so the oracle is built with that configuration too.  What is checked:
 
-- the fuzz rounds of tests/test_kernel_fuzz.py (rich generator, host events for the host paths) through step,
+- the fuzz rounds of tests/fuzz_lib.py (rich generator, host events for the host paths) through step,
   step_host, submit / submit_host + collect one and two calls deep: records and notes in order, every row as raw
   ra_row_state bytes read back through read_rows, the counters map;
 - outputs beyond the shim's first guess of their size, through step and through two calls in flight (the re-fetch and
@@ -28,11 +28,10 @@ import threading
 
 import pytest
 
-import test_call_paths_fuzz as cp
-import test_emu_fuzz as fz
-import test_kernel_fuzz as kf
+from fuzz_lib import ROLES, batch, first_row, fuzz_round, host_event, random_state, rich_event, same_keys
 from oracle_lib import Oracle
 from ra_b200 import abi
+from ra_suite import clone
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STUB = os.path.join(ROOT, "tests", "nif_stub")
@@ -239,7 +238,7 @@ def oracle(G, m):
 
 
 def o_step(o, evs):
-    msgs, notes = o.step([fz._copy(e) for e in evs], o.n_rows * abi.RA_MSG_CAP, o.n_rows * abi.RA_NOTE_CAP)
+    msgs, notes = o.step([clone(e) for e in evs], o.n_rows * abi.RA_MSG_CAP, o.n_rows * abi.RA_NOTE_CAP)
     return [x.key() for x in msgs], [x.key() for x in notes]
 
 
@@ -247,18 +246,15 @@ def same_state(eng, o, what):
     got, want = eng.rows_bytes(), o.rows_bytes()
     assert isinstance(got, bytes), "%s: read_rows returned %r" % (what, got)
     if got != want:
-        raise AssertionError("%s: rows differ from row %d" % (what, kf._first_row(want, got)))
+        raise AssertionError("%s: rows differ from row %d" % (what, first_row(want, got)))
     assert eng.counters() == o.counters(), "%s: counters" % what
 
 
 def same_out(got, want, what):
     got = outputs(got)
     assert isinstance(got, tuple) and isinstance(got[0], list), "%s: %r" % (what, got)
-    for k, (g, w) in enumerate(zip(got, want)):
-        if g != w:
-            i = next((i for i, (x, y) in enumerate(zip(w, g)) if x != y), min(len(w), len(g)))
-            raise AssertionError("%s: %s differ from #%d: oracle %r, shim %r (%d / %d)"
-                                 % (what, ("msgs", "notes")[k], i, w[i:i + 1], g[i:i + 1], len(w), len(g)))
+    for k, g, w in zip(("msgs", "notes"), got, want):
+        same_keys(w, g, what, k)
 
 
 # ---- a. the fuzz through the NIF ------------------------------------------------------------------------------------
@@ -268,25 +264,25 @@ LANES = [("step", 1), ("step_host", 1), ("submit", 1), ("submit_host", 1), ("sub
 def _lane(nif, path, depth, m, G, rounds, seed):
     rng = random.Random(seed)
     host = path.endswith("host")
-    draw = cp.host_event if host else cp._rich
+    draw = host_event if host else rich_event
     o, eng = oracle(G, m), NifEngine(nif, G, m)
     cov = dict(calls=0, beyond_guess=0)
     for rnd in range(rounds):
         # (the shim has no load_query_state: a loaded member starts with a zero query state on both sides)
-        loads, _, events = kf._fuzz_round(rng, o, m, G, rnd, draw=draw)
+        loads, _, events = fuzz_round(rng, o, rnd, draw)
         if rnd % 2:
             # every slot-0 member a leader with a deferred pipeline pass, and an empty first batch: the outputs overrun
             # the shim's first guess (its re-fetch, and the re-submission of the call behind)
             byrow = {s.row: s for s in loads}
             for r in range(G):
-                byrow[r] = fz.random_state(rng, r, G, m, abi.LEADER, rich=True)
+                byrow[r] = random_state(rng, r, G, m, abi.LEADER, rich=True)
                 byrow[r].flags |= 1
             loads, events = [byrow[r] for r in sorted(byrow)], []
         o.load_rows(loads)
         assert eng.load_rows(loads) == "ok"
         fly = []
         for t in range(3):
-            evs = events if t == 0 else cp._batch(rng, o, m, G, draw, rng.choice([0.0, 0.01, 0.3, 1.0]))
+            evs = events if t == 0 else batch(rng, o, draw, rng.choice([0.0, 0.01, 0.3, 1.0]))
             want = o_step(o, evs)
             what = "M=%d %s depth %d round %d batch %d" % (m, path, depth, rnd, t)
             cov["calls"] += 1
@@ -345,7 +341,7 @@ def _pipelined_leaders(rng, G, m):
     rows = []
     for r in range(G * m):
         role = abi.LEADER if r < G else rng.choice([abi.FOLLOWER, abi.CANDIDATE, abi.PRE_VOTE, abi.AWAIT_CONDITION])
-        s = fz.random_state(rng, r, G, m, role, rich=True)
+        s = random_state(rng, r, G, m, role, rich=True)
         if role == abi.LEADER:
             s.flags |= 1
         rows.append(s)
@@ -406,11 +402,11 @@ def _bad_batches(G, m):
 
 def _rejected(nif, G, m, seed):
     rng = random.Random(seed)
-    rows = [fz.random_state(rng, r, G, m, rng.choice(fz.ROLES), rich=True) for r in range(G * m)]
+    rows = [random_state(rng, r, G, m, rng.choice(ROLES), rich=True) for r in range(G * m)]
     o, eng = oracle(G, m), NifEngine(nif, G, m)
     o.load_rows(rows)
     assert eng.load_rows(rows) == "ok"
-    good = lambda: [cp.host_event(rng, s, m) for s in o.read_rows(range(0, G * m, 3))]
+    good = lambda: [host_event(rng, s, m) for s in o.read_rows(range(0, G * m, 3))]
     for what, code, bad in _bad_batches(G, m):
         before = eng.rows_bytes()
         assert eng.step(bad) == ("error", code), what
@@ -486,7 +482,7 @@ def _lifetime(nif, G, m, state, seed):
     rows = _pipelined_leaders(rng, G, m)
     eng = NifEngine(nif, G, m)
     assert eng.load_rows(rows) == "ok"
-    evs = [cp.host_event(rng, s, m) for s in rows[::2]]
+    evs = [host_event(rng, s, m) for s in rows[::2]]
     if state == "capacity":
         o = oracle(G, m)
         o.load_rows(rows)
@@ -494,7 +490,7 @@ def _lifetime(nif, G, m, state, seed):
         assert eng.submit([]) == "ok"
     for _ in range({"idle": 0, "one_in_flight": 1, "two_in_flight": 2, "capacity": 0}[state]):
         assert eng.submit_host(evs) == "ok"
-        evs = [cp.host_event(rng, s, m) for s in rows[1::2]]
+        evs = [host_event(rng, s, m) for s in rows[1::2]]
     assert nif.counts()["resources"] == base["resources"] + 1
     eng.drop()
     now = nif.counts()
@@ -509,7 +505,7 @@ def _lifetime(nif, G, m, state, seed):
     for x in (eng, o):
         x.load_rows(rows)
     for t in range(3):
-        evs = [cp.host_event(rng, s, m) for s in o.read_rows(range(t, G * m, 2))]
+        evs = [host_event(rng, s, m) for s in o.read_rows(range(t, G * m, 2))]
         assert eng.submit_host(evs) == "ok"
         same_out(eng.collect(), o_step(o, evs), "%s: next engine, step %d" % (state, t))
     same_state(eng, o, state)
@@ -532,10 +528,10 @@ def test_engine_dropped_with_calls_in_flight_engine(nif_gpu):
 def _thread_plan(k, G, m, rounds):
     """thread k's engine: its rows and 2 * rounds host-event batches"""
     rng = random.Random(17000 + k)
-    rows = [fz.random_state(rng, r, G, m, rng.choice(fz.ROLES), rich=True) for r in range(G * m)]
+    rows = [random_state(rng, r, G, m, rng.choice(ROLES), rich=True) for r in range(G * m)]
     batches = []
     for _ in range(2 * rounds):
-        batches.append([cp.host_event(rng, s, m) for s in rows if rng.random() < 0.3])
+        batches.append([host_event(rng, s, m) for s in rows if rng.random() < 0.3])
     return rows, batches
 
 

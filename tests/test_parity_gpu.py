@@ -7,11 +7,10 @@
  * size-independent properties at full size (commit monotonic, commit <= last_index, one
    leader per term, followers' logs are prefixes of the leader's term view).
 """
-import ctypes as C
-
 import pytest
 
 import trace_gen
+from fuzz_lib import bootstrap, first_row
 from oracle_lib import Oracle
 from ra_b200 import abi
 
@@ -63,19 +62,6 @@ def test_trace_parity_small_pipeline_window():
     assert got == want and got_rows == want_rows and got_cnt == want_cnt
 
 
-def _first_diff(a: bytes, b: bytes) -> int:
-    sz = C.sizeof(abi.RaRowState)
-    for i in range(0, len(a), sz):
-        if a[i:i + sz] != b[i:i + sz]:
-            return i // sz
-    return -1
-
-
-def _bootstrap(b):
-    b.reset_empty()
-    b.step([abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(b.n_groups)])
-
-
 FLOODS = [
     (64, 3, 60, 1, 0),       # config 1 shape, clean
     (1000, 5, 80, 1, 0),
@@ -92,7 +78,7 @@ def test_flood_parity(g, m, steps, cmds, permille):
     o = Oracle(g, m, route_on_device=True)
     e = _engine(g, m, route_on_device=True)
     for b in (o, e):
-        _bootstrap(b)
+        bootstrap(b)
     # several calls so that the step counter / buffer parity carry over
     for part in (steps // 3, steps - steps // 3):
         o.flood(part, cmds, permille, seed=42, threads=8)
@@ -101,7 +87,7 @@ def test_flood_parity(g, m, steps, cmds, permille):
     assert ce == co
     assert co["commits"] > 0
     ro, re_ = o.rows_bytes(), e.rows_bytes()
-    assert re_ == ro, "first differing row: %d" % _first_diff(ro, re_)
+    assert re_ == ro, "first differing row: %d" % first_row(ro, re_)
 
 
 def test_flood_parity_full_size_and_properties():
@@ -110,14 +96,14 @@ def test_flood_parity_full_size_and_properties():
     o = Oracle(g, m, route_on_device=True)
     e = _engine(g, m, route_on_device=True)
     for b in (o, e):
-        _bootstrap(b)
+        bootstrap(b)
         if b is o:
             b.flood(steps, 1, 10, seed=9, threads=8)
         else:
             b.flood(steps, 1, 10, seed=9)
     assert e.counters() == o.counters()
     ro, re_ = o.rows_bytes(), e.rows_bytes()
-    assert re_ == ro, "first differing row: %d" % _first_diff(ro, re_)
+    assert re_ == ro, "first differing row: %d" % first_row(ro, re_)
     # properties on the engine's rows (sampled groups)
     rows = e.read_rows([e.row_of(gg, s) for gg in range(0, g, 997) for s in range(m)])
     for i in range(0, len(rows), m):
@@ -164,9 +150,9 @@ def test_host_driven_flood_equals_device_flood():
     a = _engine(g, m, route_on_device=True)
     b = _engine(g, m, route_on_device=True)
     o = Oracle(g, m, route_on_device=True)
-    _bootstrap(a)
+    bootstrap(a)
     a.flood(steps, 1, 10, seed=5)
-    _bootstrap(o)
+    bootstrap(o)
     o.flood(steps, 1, 10, seed=5, threads=8)
     b.reset_empty()
     hf = HostFlood(b)
@@ -177,4 +163,4 @@ def test_host_driven_flood_equals_device_flood():
     for k in ("events", "commits", "applied", "msgs_out", "elections_won"):
         assert cb[k] == ca[k]
     ra, rb = a.rows_bytes(), b.rows_bytes()
-    assert rb == ra, "first differing row: %d" % _first_diff(ra, rb)
+    assert rb == ra, "first differing row: %d" % first_row(ra, rb)

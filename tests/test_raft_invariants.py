@@ -48,7 +48,7 @@ import pytest
 import trace_gen
 from emu_lib import Emu
 from ra_b200 import abi
-from ra_suite import make_backend
+from ra_suite import clone, make_backend
 
 LIM = 1 << 30
 BIG = 1 << 62
@@ -551,7 +551,7 @@ def run_closed_loop(b, steps, seed, pure=False, p_restart=0.03, min_restarts=3, 
         if pure:                                            # {next_event, _}: to the member itself, first
             nxt = [x for x in msgs if x.flags & abi.EVF_NEXT_EVENT]
             for x in reversed(nxt):
-                e = trace_gen.copy_ev(x)
+                e = clone(x)
                 e.flags &= ~abi.EVF_NEXT_EVENT
                 cl.queues[e.row].appendleft(e)
             msgs = [x for x in msgs if not x.flags & abi.EVF_NEXT_EVENT]
@@ -758,7 +758,7 @@ class Script:
             self.host.check_applied(self.chk, "script step %d" % self.t)
             for x in msgs:
                 if x.row in self.up and link(x.from_slot, x.row, x):
-                    self.mail.append(trace_gen.copy_ev(x))
+                    self.mail.append(clone(x))
             for n in notes:
                 if n.type == abi.NOTE_WAL_APPEND and n.row in self.up:
                     w = abi.ev_written(n.row, n.c, n.a, n.b)
@@ -909,7 +909,7 @@ def test_append_entries_longer_than_65535(backend, runs, last, routed, monkeypat
             if x.type == abi.EV_AER:
                 assert x.n >= x.n1 and x.a + x.n <= last, "step %d: AppendEntries prev %d n %d n1 %d, leader last %d" % (
                     t, x.a, x.n, x.n1, last)
-            mail.append(trace_gen.copy_ev(x))
+            mail.append(clone(x))
         for n in notes:
             if n.type == abi.NOTE_WAL_APPEND:
                 w = abi.ev_written(n.row, n.c, n.a, n.b)

@@ -10,27 +10,24 @@ steps also every record and note.
 
 CPU tier: the host emulation (tests/emu) reads the bytes the kernel would not have fetched as poison and counts every
 record it decoded from them (Emu.underfetched), so a lost flag shows there.  Each case has a twin at reduced size on
-the plane-stats build (test_short_records.stats_lib()) that asserts the precondition: the targeted records really were
+the plane-stats build (emu_lib.stats_lib()) that asserts the precondition: the targeted records really were
 stored as heads (or long).  GPU tier: the same cases on the engine, with the 32-bit (RA_STEP_WIDE=0) and the 64-bit
 (RA_STEP_WIDE=1) hot kernel.
 """
-import ctypes as C
 import functools
 from collections import defaultdict
 
 import pytest
 
 import trace_gen
-from emu_lib import Emu, EmuShards
+from emu_lib import Emu, EmuShards, plane_forms, stats_lib
+from fuzz_lib import WIDTHS, bootstrap, first_row
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_suite import make_backend
-from test_short_records import plane_forms, stats_lib
 
 BACKENDS = ["emu", pytest.param("engine", marks=pytest.mark.gpu)]
-WIDTHS = ["0", "1"]                       # RA_STEP_WIDE: the 32-bit hot kernel / the 64-bit one
 PERMILLE, SEED = 15, 0x5EC
-SHORT, HEAD, LONG = 0, 1, 2                 # positions in the (short, head, long) counts of plane_forms()
 
 
 @pytest.fixture(autouse=True)
@@ -56,20 +53,13 @@ def _check_fetch(name):
 
 
 def _same_rows(got, want):
-    sz = C.sizeof(abi.RaRowState)
     a, b = got.rows_bytes(), want.rows_bytes()
-    first = next((i // sz for i in range(0, len(a), sz) if a[i:i + sz] != b[i:i + sz]), -1)
-    assert a == b, "first differing row: %d" % first
+    assert a == b, "first differing row: %d" % first_row(a, b)
 
 
 def _keys(out):
     msgs, notes = out
     return [m.key() for m in msgs], [n.key() for n in notes]
-
-
-def _bootstrap(b):
-    b.reset_empty()
-    b.step([abi.ev_simple(b.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(b.n_groups)])
 
 
 # ---- floods: mailbox planes (emit_msg, row_end_of_step) and host planes (the flood host model) ----------------------
@@ -90,7 +80,7 @@ FLOOD_IDS = ["m%d-c%d-b%d%s" % (m, c, b, "-faults" if f else "") for m, c, b, f 
 
 def _flood(b, o, steps, cmds, faults):
     for x in (o, b):
-        _bootstrap(x)
+        bootstrap(x)
     o.flood(steps, cmds, PERMILLE, seed=SEED, threads=4, faults=faults)
     b.flood(steps, cmds, PERMILLE, seed=SEED, faults=faults)
 
@@ -112,23 +102,23 @@ def test_flood_with_head_and_long_records(members, cmds, batch, faults, backend,
 @pytest.mark.parametrize("members,cmds,batch,faults", FLOODS, ids=FLOOD_IDS)
 def test_flood_with_head_and_long_records_twin(members, cmds, batch, faults):
     e = Emu(48, members, library=stats_lib(), route_on_device=True, max_aer_batch=batch)
-    _bootstrap(e)
+    bootstrap(e)
     plane_forms()
     e.flood(40, cmds, PERMILLE, SEED, faults)
     forms = plane_forms()
     assert Emu.underfetched(library=stats_lib()) == 0
     assert e.counters()["commits"] > 0
     if cmds < 256:
-        assert all(h == 0 for _, h, _ in forms.values()), forms
+        assert all(f.head == 0 for f in forms.values()), forms
         return
-    assert forms[abi.EV_COMMAND][HEAD] > 0, forms[abi.EV_COMMAND]
+    assert forms[abi.EV_COMMAND].head > 0, forms[abi.EV_COMMAND]
     if batch >= 256:
-        assert forms[abi.EV_AER][HEAD] > 0, forms[abi.EV_AER]
+        assert forms[abi.EV_AER].head > 0, forms[abi.EV_AER]
     else:                                  # 300 entries as three records per follower and step, all short
-        assert forms[abi.EV_AER][HEAD] == 0
-        assert forms[abi.EV_AER][SHORT] >= 2 * (members - 1) * forms[abi.EV_COMMAND][HEAD], forms
+        assert forms[abi.EV_AER].head == 0
+        assert forms[abi.EV_AER].short >= 2 * (members - 1) * forms[abi.EV_COMMAND].head, forms
     if faults:
-        assert forms[abi.EV_AER][LONG] > 0, forms[abi.EV_AER]
+        assert forms[abi.EV_AER].long > 0, forms[abi.EV_AER]
 
 
 # ---- closed-loop traces, not routed: RPC records return as host events (ingest_kernel) ------------------------------
@@ -163,7 +153,7 @@ def test_trace_with_long_batches_twin(members):
     _replay_equal(Emu(10, members, library=stats_lib(), max_aer_batch=512), members)
     forms = plane_forms()
     assert Emu.underfetched(library=stats_lib()) == 0
-    assert forms[abi.EV_COMMAND][HEAD] > 0 and forms[abi.EV_AER][HEAD] > 0, forms
+    assert forms[abi.EV_COMMAND].head > 0 and forms[abi.EV_AER].head > 0, forms
 
 
 # ---- one scripted step batch: every form in the same host slot of every tile ----------------------------------------
@@ -181,7 +171,7 @@ def _scripted_kinds(row):
 
 
 def _scripted(b):
-    _bootstrap(b)
+    bootstrap(b)
     out = []
     for shift in (0, 3, 5):
         batch = []
@@ -211,9 +201,9 @@ def test_scripted_step_mixes_every_form_in_a_tile_twin():
     _scripted(e)
     forms = plane_forms()
     assert Emu.underfetched(library=stats_lib()) == 0
-    assert forms[abi.EV_COMMAND][SHORT] > 0 and forms[abi.EV_COMMAND][HEAD] > 0, forms[abi.EV_COMMAND]
-    assert forms[abi.EV_AER][HEAD] > 0 and forms[abi.EV_AER][LONG] > 0, forms[abi.EV_AER]
-    assert forms[abi.EV_AER_REPLY][HEAD] > 0 and forms[abi.EV_PRE_VOTE][LONG] > 0, forms
+    assert forms[abi.EV_COMMAND].short > 0 and forms[abi.EV_COMMAND].head > 0, forms[abi.EV_COMMAND]
+    assert forms[abi.EV_AER].head > 0 and forms[abi.EV_AER].long > 0, forms[abi.EV_AER]
+    assert forms[abi.EV_AER_REPLY].head > 0 and forms[abi.EV_PRE_VOTE].long > 0, forms
 
 
 # ---- step_host: 32-byte host events through ingest_kernel<ra_host_event>, closed loop over a routed engine ---------
@@ -268,9 +258,9 @@ def test_step_host_long_commands_and_wide_written_twin(wide_values):
     _host_loop(e, wide_values)
     forms = plane_forms()
     assert Emu.underfetched(library=stats_lib()) == 0
-    assert forms[abi.EV_COMMAND][HEAD] > 0 and forms[abi.EV_AER][HEAD] > 0, forms
+    assert forms[abi.EV_COMMAND].head > 0 and forms[abi.EV_AER].head > 0, forms
     if wide_values:
-        assert forms[abi.EV_WRITTEN][HEAD] > 0 and forms[abi.EV_WRITTEN][SHORT] == 0, forms[abi.EV_WRITTEN]
+        assert forms[abi.EV_WRITTEN].head > 0 and forms[abi.EV_WRITTEN].short == 0, forms[abi.EV_WRITTEN]
 
 
 # ---- sharded: bucket transport (deliver_record's CAS) and peer stores against the unsharded oracle ------------------
@@ -280,7 +270,7 @@ SHARDED = [(2, 5, 300), (8, 5, 64)]          # shards, members, local groups per
 def _sharded_oracle(n, m, gl, steps):
     g = n * gl
     o = Oracle(g, m, route_on_device=True, max_aer_batch=512)
-    _bootstrap(o)
+    bootstrap(o)
     o.flood(steps, 300, PERMILLE, seed=SEED, threads=8)
     return o, {r.row: r.key()[1:] for r in o.read_rows(range(o.n_rows))}
 
@@ -334,7 +324,7 @@ def test_sharded_buckets_with_head_records_emu(n, m, gl):
 def _stall_crossing(b):
     """Leaders take a 300-entry command in the hot kernel (head AppendEntries to every follower), then stall on a reply
     from an unknown slot; the step after, the followers read those heads in the hot kernel."""
-    _bootstrap(b)
+    bootstrap(b)
     out = []
     for _ in range(4):                                       # elections complete; the leaders' noop entries replicate
         out.append(_keys(b.step([])))
@@ -367,5 +357,5 @@ def test_head_record_sent_before_a_stall_twin():
     _stall_crossing(e)
     forms = plane_forms()
     assert Emu.underfetched(library=stats_lib()) == 0
-    assert forms[abi.EV_AER][HEAD] >= 4 * 64, forms[abi.EV_AER]
+    assert forms[abi.EV_AER].head >= 4 * 64, forms[abi.EV_AER]
     assert Emu.stall_stats(library=stats_lib())["stalls_wk_hi"] >= 64

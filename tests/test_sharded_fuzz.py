@@ -21,26 +21,18 @@ which record an overflowing bucket loses depends on the order of the kernel's at
 (tests/test_sharded_gpu.py checks that an overflow is counted).
 """
 import ctypes as C
-import random
 
 import pytest
 
-import test_emu_fuzz as fz
 from emu_lib import Emu, EmuShards
+from fuzz_lib import MODES, NOTE_CAPS, budget_coverage, fuzz_rounds, kw, widths
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_b200.sharded import global_group, local_group, shard_of
-from test_kernel_fuzz import (FAULTS, FLOOD_CMDS, MODES, NOTE_CAPS, PERMILLE, WIDTHS, _budget_coverage, _compare,
-                              _fuzz_round, _kw, _observe, _snapshot_bursts, _unconsumed)
+from ra_suite import clone
 
 TRANSPORTS = ["buckets", "peer"]
 SHARD_MODES = ["routed", "flood"]                # sharding routes on the device
-
-
-def _clone(x):
-    d = type(x)()
-    C.memmove(C.byref(d), C.byref(x), C.sizeof(x))
-    return d
 
 
 def _bucket_cap(groups_local, m):
@@ -72,7 +64,7 @@ class Sharded:
         per = [[] for _ in self.shards]
         for x in items:
             k, lr = self.where[x.row]
-            y = _clone(x)
+            y = clone(x)
             y.row = lr
             per[k].append(y)
         return per
@@ -147,60 +139,12 @@ class Sharded:
                 tot[k] = tot.get(k, 0) + v
         return tot
 
-    def observe(self, m, out):
-        msgs, notes = out
-        return dict(msgs=[x.key() for x in msgs], notes=[x.key() for x in notes], rows=self.rows_bytes(),
-                    counters=self.counters(), query=[x.key(m) for x in self.read_query_state(range(self.n_rows))])
-
 
 def _fuzz_sharded(bs, mode, m, G, rounds, seed, note_cap=0):
-    """bs: Sharded backends over G groups; each is stepped with the oracle and compared with it after every step.
-    note_cap != 0: the host events a budget left unconsumed are submitted again (test_kernel_fuzz._fuzz)."""
-    rng = random.Random(seed)
-    o = Oracle(G, m, **_kw(mode, note_cap))
-    cov = dict(refused=0, fatal_overflow=0, fault_drops=0)
-    for rnd in range(rounds):
-        loads, qs, events = _fuzz_round(rng, o, m, G, rnd)
-        if note_cap:
-            _snapshot_bursts(rng, loads, m)
-        steps = [events] + ([[], []] if mode == "routed" else [])
-        for x in [o] + bs:
-            x.load_rows(loads)
-            x.load_query_state(qs)
-
-        def check(what, outs, evs):
-            want = _observe(o, m, out=outs[0])
-            for b, out in zip(bs, outs[1:]):
-                _compare(want, b.observe(m, out), "N=%d M=%d %s round %d %s: %s" % (b.n, m, mode, rnd, b.label, what),
-                         evs, o)
-
-        k = 0
-        while k < len(steps):
-            evs = steps[k]
-            outs = [x.step([fz._copy(e) for e in evs]) for x in [o] + bs]
-            check("step %d" % k, outs, evs)
-            left = _unconsumed(outs[0][1], evs)
-            cov["refused"] += len(left)
-            cov["fatal_overflow"] += sum(1 for n in outs[0][1] if n.type == abi.NOTE_STATUS and n.aux & abi.ST_FATAL
-                                         and n.c & 0xff == abi.FATAL_NOTE_OVERFLOW)
-            if left:
-                if k + 1 < len(steps):
-                    steps[k + 1] = left + steps[k + 1]
-                else:
-                    steps.append(left)
-            k += 1
-        if mode == "flood":
-            faults = FAULTS if rnd % 2 else None
-            for t in range(4):                                  # F.step carries over: four 1-step floods = one of 4
-                dropped = o.counters()["msgs_dropped"]
-                o.flood(1, FLOOD_CMDS, PERMILLE, seed=seed + rnd, threads=4, faults=faults)
-                for b in bs:
-                    b.flood(1, FLOOD_CMDS, PERMILLE, seed=seed + rnd, faults=faults)
-                check("flood%s step %d" % (" with faults" if faults else "", t), [([], [])] * (1 + len(bs)), [])
-                if faults:
-                    cov["fault_drops"] += o.counters()["msgs_dropped"] - dropped
-            outs = [x.step([]) for x in [o] + bs]
-            check("the step after the flood", outs, [])
+    """bs: Sharded backends over G groups, each stepped with the unsharded oracle and compared with it after every step
+    and after each step of a flood -> (oracle, coverage)."""
+    o = Oracle(G, m, **kw(mode, note_cap))
+    cov = fuzz_rounds(o, [(b.label, b) for b in bs], mode, rounds, seed, note_cap=note_cap, flood_chunk=1)
     assert o.counters()["fatal_rows"] > 0
     if mode == "flood" and rounds > 1:
         assert cov["fault_drops"] > 0, "the faulted floods dropped no record"
@@ -208,14 +152,13 @@ def _fuzz_sharded(bs, mode, m, G, rounds, seed, note_cap=0):
 
 
 # ---- CPU tier: shards of the host emulation ---------------------------------------------------------------------
-def _emu_sharded(transport, n, G, m, monkeypatch, **kw):
-    kw.pop("route_on_device")
+def _emu_sharded(transport, n, G, m, monkeypatch, **cfg):
+    cfg.pop("route_on_device")
     gl = G // n
     out = []
-    for w in WIDTHS:
-        monkeypatch.setenv("RA_STEP_WIDE", w)                 # read when the shards are created
-        es = EmuShards(n, gl, m, cap=_bucket_cap(gl, m), peer=(transport == "peer"), **kw)
-        out.append(Sharded(es.shards, es.exchange, G, m, "emu %s RA_STEP_WIDE=%s" % (transport, w), keep=es))
+    for w in widths(monkeypatch):
+        es = EmuShards(n, gl, m, cap=_bucket_cap(gl, m), peer=(transport == "peer"), **cfg)
+        out.append(Sharded(es.shards, es.exchange, G, m, "N=%d emu %s RA_STEP_WIDE=%s" % (n, transport, w), keep=es))
     return out
 
 
@@ -236,7 +179,7 @@ EMU_SHAPES = [(2, 5), (3, 5), (2, 3), (3, 7), (8, 5), (4, 4), (5, 8), (8, 3)]   
 def test_sharded_fuzz_emu(n, m, mode, transport, monkeypatch):
     G = 40 if n == 5 else 48
     Emu.narrow_stats(); Emu.stall_stats(); Emu.underfetched()
-    bs = _emu_sharded(transport, n, G, m, monkeypatch, **_kw(mode))
+    bs = _emu_sharded(transport, n, G, m, monkeypatch, **kw(mode))
     _fuzz_sharded(bs, mode, m, G, 6, 9000 + 100 * n + 10 * m + SHARD_MODES.index(mode))
     _emu_coverage(transport, m)
 
@@ -251,28 +194,27 @@ def test_sharded_fuzz_note_cap_emu(n, m, mode, transport, monkeypatch):
     G = 48
     cap = NOTE_CAPS[m][MODES.index(mode)]
     Emu.narrow_stats(); Emu.stall_stats(); Emu.underfetched()
-    bs = _emu_sharded(transport, n, G, m, monkeypatch, **_kw(mode, cap))
+    bs = _emu_sharded(transport, n, G, m, monkeypatch, **kw(mode, cap))
     o, cov = _fuzz_sharded(bs, mode, m, G, 6, 9500 + 100 * n + 10 * m, cap)
-    _budget_coverage(o, m, mode, cov)
+    budget_coverage(o, m, mode, cov)
     assert Emu.underfetched() == 0
 
 
 # ---- GPU tier: ra_b200.sharded.Shard, bucket and peer transports, the 32-bit and the 64-bit hot kernel --------------
-def _engine_sharded(transports, n, G, m, monkeypatch, **kw):
+def _engine_sharded(transports, n, G, m, monkeypatch, **cfg):
     """Never a device-side barrier here: all shards share one stream, a barrier kernel would wait for shards that
     cannot run.  The host steps the shards in turn instead."""
     from ra_b200.sharded import LocalPeerTransport, LocalTransport, Shard
-    kw.pop("route_on_device")
+    cfg.pop("route_on_device")
     gl = G // n
     out = []
     for transport in transports:
-        for w in WIDTHS:
-            monkeypatch.setenv("RA_STEP_WIDE", w)             # read when the engines are created
-            shards = [Shard(gl, m, n, k, cap=_bucket_cap(gl, m), buckets=(transport == "buckets"), **kw)
+        for w in widths(monkeypatch):
+            shards = [Shard(gl, m, n, k, cap=_bucket_cap(gl, m), buckets=(transport == "buckets"), **cfg)
                       for k in range(n)]
             t = LocalTransport(shards) if transport == "buckets" else LocalPeerTransport(shards)
-            out.append(Sharded([s.eng for s in shards], t.exchange, G, m, "engine %s RA_STEP_WIDE=%s" % (transport, w),
-                               keep=(shards, t)))
+            out.append(Sharded([s.eng for s in shards], t.exchange, G, m,
+                               "N=%d engine %s RA_STEP_WIDE=%s" % (n, transport, w), keep=(shards, t)))
     return out
 
 
@@ -284,7 +226,7 @@ GPU_SHAPES = [(2, 5), (8, 5), (5, 5), (3, 7), (4, 3), (8, 8)]          # (5, 5):
 @pytest.mark.parametrize("n,m", GPU_SHAPES)
 def test_sharded_fuzz_engine(n, m, mode, monkeypatch):
     G = 1200
-    bs = _engine_sharded(TRANSPORTS, n, G, m, monkeypatch, **_kw(mode))
+    bs = _engine_sharded(TRANSPORTS, n, G, m, monkeypatch, **kw(mode))
     _fuzz_sharded(bs, mode, m, G, 3, 9700 + 100 * n + 10 * m + SHARD_MODES.index(mode))
     for b in bs:
         assert b.stall_histogram(), "%s: no row took the general kernel" % b.label
@@ -298,6 +240,6 @@ GPU_BUDGET_CASES = [("buckets", 3, 7, "routed"), ("peer", 2, 5, "flood")]
 def test_sharded_fuzz_note_cap_engine(transport, n, m, mode, monkeypatch):
     G = 1200
     cap = NOTE_CAPS[m][MODES.index(mode)]
-    bs = _engine_sharded([transport], n, G, m, monkeypatch, **_kw(mode, cap))
+    bs = _engine_sharded([transport], n, G, m, monkeypatch, **kw(mode, cap))
     o, cov = _fuzz_sharded(bs, mode, m, G, 2, 9900 + 100 * n + 10 * m, cap)
-    _budget_coverage(o, m, mode, cov)
+    budget_coverage(o, m, mode, cov)

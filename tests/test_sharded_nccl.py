@@ -3,23 +3,16 @@ buckets travel by NCCL all_to_all_single; every rank checks its members against 
 oracle run.  Skipped on a single-GPU box (the same kernels/ABI are covered there by
 tests/test_sharded_gpu.py with the in-process transport)."""
 import os
-import socket
 import subprocess
 import sys
 import textwrap
 
 import pytest
 
+from fuzz_lib import free_port
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 @pytest.mark.parametrize("transport", ["a2a", "peer", "peer-devbar"])
@@ -68,7 +61,7 @@ def test_nccl_sharded_flood_equals_oracle(world, transport, tmp_path):
     """ % (ROOT, ROOT, transport, transport)))
     env = dict(os.environ, MASTER_ADDR="127.0.0.1")
     out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(world),
-                          "--master-addr", "127.0.0.1", "--master-port", str(_free_port()), str(script)],
+                          "--master-addr", "127.0.0.1", "--master-port", str(free_port()), str(script)],
                          capture_output=True, text=True, env=env, timeout=600)
     assert out.returncode == 0, out.stderr[-3000:]
     line = [ln for ln in out.stdout.splitlines() if ln.startswith("RESULT")][-1].split()

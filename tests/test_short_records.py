@@ -4,48 +4,15 @@ A record whose fields fit is stored in chunk 0 of its tile alone; everything els
 64-byte long form.  Checked here through the host emulation of the device logic: round trips through both index
 widths at every limit of the short form, stale bytes in chunks 1..3 of the tile, and -- at the shapes of the
 benchmark's configurations -- that every record the steady state writes into a plane is short."""
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import pytest
 
-from emu_lib import Emu
+from emu_lib import HEAD, LONG, SHORT, Emu, extras, plane_forms, stats_lib
+from fuzz_lib import bootstrap
 from ra_b200 import abi
 
-SHORT, HEAD, LONG = 0, 1, 3          # what st_rec_plane reports: nothing but chunk 0 / chunks 0-1 / chunks 0-3
 NARROW_LIMIT = 1 << 30
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu", "plane_stats.cpp")
-_lib_cache = []
-
-
-def stats_lib():
-    """tests/emu/plane_stats.cpp: the host emulation built with per-form store counters, compiled on first use into a
-    temporary directory (the tree is left as it is).  Emu(..., library=stats_lib()) runs on it."""
-    if _lib_cache:
-        return _lib_cache[0]
-    d = tempfile.mkdtemp(prefix="ra_plane_stats_")
-    atexit.register(shutil.rmtree, d, True)
-    so = os.path.join(d, "libra_plane_stats.so")
-    subprocess.check_call([os.environ.get("CXX", "g++"), "-O1", "-std=c++17", "-fPIC", "-shared", "-Wl,-Bsymbolic",
-                           "-Wl,--no-undefined", "-o", so, _SRC])
-    _lib_cache.append(C.CDLL(so))
-    return _lib_cache[0]
-
-
-_int_p = C.POINTER(C.c_int)
-EXTRAS = {                                     # ra_emu_<name> of the plane-stats build
-    "codec_roundtrip2": (C.c_int, [C.POINTER(abi.RaEvent), C.c_int, C.POINTER(abi.RaEvent), _int_p,
-                                   C.POINTER(abi.RaEvent), _int_p, _int_p]),
-    "plane_forms": (None, [C.POINTER(C.c_ulonglong), C.c_int]),
-}
-
-
-def _stats():
-    return abi.bind(stats_lib(), "ra_emu", EXTRAS)
 
 
 def _fields(e):
@@ -58,8 +25,8 @@ def roundtrip(e, want_form):
     for fill in (0x00, 0xA5, 0xFF):
         ow, on = abi.RaEvent(), abi.RaEvent()
         form, fits, form_n = C.c_int(-1), C.c_int(-1), C.c_int(-1)
-        assert _stats().codec_roundtrip2(C.byref(e), fill, C.byref(ow), C.byref(form), C.byref(on), C.byref(fits),
-                                         C.byref(form_n)) == 0
+        assert extras(stats_lib()).codec_roundtrip2(C.byref(e), fill, C.byref(ow), C.byref(form), C.byref(on),
+                                                    C.byref(fits), C.byref(form_n)) == 0
         assert form.value == want_form, (fill, _fields(e))
         assert _fields(ow) == _fields(e) and ow._pad == 0, (fill, _fields(ow), _fields(e))
         # the narrow pass refuses every record with a field >= 2^30, in any form
@@ -127,19 +94,13 @@ def test_random_records_roundtrip():
                         c=rng.choice([t, 0, rng.choice(vals)]), d=rng.choice([0, 1, t]), e=rng.choice([0, 0, 5]))
         ow, on = abi.RaEvent(), abi.RaEvent()
         form, fits, form_n = C.c_int(-1), C.c_int(-1), C.c_int(-1)
-        assert _stats().codec_roundtrip2(C.byref(e), rng.randrange(256), C.byref(ow), C.byref(form), C.byref(on),
-                                         C.byref(fits), C.byref(form_n)) == 0
+        assert extras(stats_lib()).codec_roundtrip2(C.byref(e), rng.randrange(256), C.byref(ow), C.byref(form),
+                                                    C.byref(on), C.byref(fits), C.byref(form_n)) == 0
         assert _fields(ow) == _fields(e)
         if fits.value:
             assert _fields(on) == _fields(e) and form_n.value == form.value
         if form.value == SHORT:
             assert max(e.term, e.a, e.b, e.c, e.d, e.e) < 2**32 and e.n < 256 and e.n1 < 256 and e.flags < 16
-
-
-def plane_forms():
-    arr = (C.c_ulonglong * 64)()
-    _stats().plane_forms(arr, 1)
-    return {t: (arr[4 * t + SHORT], arr[4 * t + HEAD], arr[4 * t + LONG]) for t in range(16)}
 
 
 # the benchmark's configurations 3, 4 and 5 at a size the emulation runs in seconds
@@ -153,18 +114,16 @@ SHAPES = [
 @pytest.mark.parametrize("shape", SHAPES, ids=["config3", "config4", "config5"])
 def test_steady_state_records_are_written_short(shape):
     e = Emu(shape["groups"], shape["members"], library=stats_lib(), route_on_device=True)
-    e.reset_empty()
-    e.step([abi.ev_simple(e.row_of(g, 0), abi.EV_ELECTION_TIMEOUT) for g in range(shape["groups"])])
+    bootstrap(e)
     e.flood(20, shape["cmds"], shape["permille"], seed=0xA03, faults=shape["faults"])
     plane_forms()                                                              # reset
     e.flood(60, shape["cmds"], shape["permille"], seed=0xA03, faults=shape["faults"])
     forms = plane_forms()
     # no record without a tail needed more than chunk 0: every AppendEntries of the leader's term, every reply,
     # written and command event (and every vote record without a tail) was written short
-    assert all(h == 0 for _, h, _ in forms.values()), forms
+    assert all(f.head == 0 for f in forms.values()), forms
     for t in (abi.EV_AER, abi.EV_AER_REPLY, abi.EV_WRITTEN, abi.EV_COMMAND):
-        short, _, long_ = forms[t]
-        assert short > 0, (t, forms[t])
-    aer_short, _, aer_long = forms[abi.EV_AER]
-    assert aer_long < 0.05 * aer_short, forms[abi.EV_AER]                    # the long ones follow leader changes
+        assert forms[t].short > 0, (t, forms[t])
+    aer = forms[abi.EV_AER]
+    assert aer.long < 0.05 * aer.short, aer                    # the long ones follow leader changes
     assert e.counters()["commits"] > 0

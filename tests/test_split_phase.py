@@ -14,43 +14,11 @@ def _cluster(be, groups=64, members=3, **kw):
     return b
 
 
-def _drive(b, steps, step_fn):
-    """a host-routed closed loop: every RPC record goes back in as an event of the next step"""
-    evs = [ev_simple(b.row_of(g, 0), EV_ELECTION_TIMEOUT) for g in range(b.n_groups)]
-    out = []
-    for t in range(steps):
-        evs.sort(key=lambda e: e.row)
-        # at most RA_LOCAL_CAP per row
-        take, rest, cnt = [], [], {}
-        for e in evs:
-            c = cnt.get(e.row, 0)
-            (take if c < 4 else rest).append(e)
-            cnt[e.row] = c + 1
-        msgs, notes = step_fn(take)
-        out.append(([m.key() for m in msgs], [n.key() for n in notes]))
-        evs = rest + [trace_copy(m) for m in msgs]
-        for n in notes:
-            if n.type == NOTE_WAL_APPEND:
-                evs.append(ev_written(n.row, n.c, n.a, n.b))
-        if t % 3 == 0:
-            rows = b.read_rows(range(b.n_rows))
-            evs += [ev_command(r.row, 1) for r in rows if r.role == LEADER]
-    return out
-
-
-def trace_copy(m):
-    e = RaEvent()
-    import ctypes as C
-    C.memmove(C.byref(e), C.byref(m), C.sizeof(m))
-    e.seq = 0
-    return e
-
-
 @pytest.mark.parametrize("be", ["emu", pytest.param("engine", marks=pytest.mark.gpu)])
 def test_output_capacity_loses_nothing(be):
     ref = _cluster(be)
     tiny = _cluster(be)
-    want = _drive(ref, 12, lambda evs: ref.step(evs))
+    want = closed_loop(ref, 12, lambda evs: ref.step(evs))
 
     def tiny_step(evs):
         try:
@@ -64,7 +32,7 @@ def test_output_capacity_loses_nothing(be):
         st, nm2, nn2, msgs, notes = tiny.fetch_output(nm, nn)
         assert st == RA_OK and (nm2, nn2) == (nm, nn)
         return msgs, notes
-    got = _drive(tiny, 12, tiny_step)
+    got = closed_loop(tiny, 12, tiny_step)
     assert got == want
     assert [r.key() for r in tiny.read_rows(range(tiny.n_rows))] == [r.key() for r in ref.read_rows(range(ref.n_rows))]
 
@@ -73,7 +41,7 @@ def test_output_capacity_loses_nothing(be):
 def test_submit_collect_equals_step():
     ref = _cluster("engine")
     sp = _cluster("engine")
-    want = _drive(ref, 15, lambda evs: ref.step(evs))
+    want = closed_loop(ref, 15, lambda evs: ref.step(evs))
 
     def split_step(evs):
         st, tk = sp.submit(evs, 4096, 4096)
@@ -81,7 +49,7 @@ def test_submit_collect_equals_step():
         st, nm, nn, msgs, notes = sp.collect(tk)
         assert st == RA_OK
         return msgs, notes
-    assert _drive(sp, 15, split_step) == want
+    assert closed_loop(sp, 15, split_step) == want
 
 
 @pytest.mark.gpu

@@ -13,13 +13,7 @@ from collections import defaultdict, deque
 from typing import Dict, List, Sequence, Tuple
 
 from ra_b200 import abi
-
-
-def copy_ev(e: abi.RaEvent) -> abi.RaEvent:
-    c = abi.RaEvent()
-    for name, _ in abi.RaEvent._fields_:
-        setattr(c, name, getattr(e, name))
-    return c
+from ra_suite import clone
 
 
 class Cluster:
@@ -122,9 +116,9 @@ class Cluster:
         for m in msgs:
             if rng.random() < self.p_drop:
                 continue
-            self._post(copy_ev(m))
+            self._post(clone(m))
             if rng.random() < self.p_dup:
-                self._post(copy_ev(m), 1, duplicate=True)
+                self._post(clone(m), 1, duplicate=True)
         saw_leader = set()
         for i, n in enumerate(notes):
             last_of_row = i + 1 == len(notes) or notes[i + 1].row != n.row
@@ -158,7 +152,7 @@ def generate(make_backend, n_groups: int, n_members: int, n_steps: int, seed: in
         batch = cl.next_batch()
         msgs, notes = b.step(batch)
         cl.absorb(msgs, notes)
-        batches.append([copy_ev(e) for e in batch])
+        batches.append([clone(e) for e in batch])
     b.close()
     return batches
 
@@ -167,7 +161,7 @@ def replay(backend, batches: Sequence[Sequence[abi.RaEvent]]):
     """Feed a recorded trace to a backend; return per-step (msgs, notes) keys and final rows."""
     out = []
     for batch in batches:
-        msgs, notes = backend.step([copy_ev(e) for e in batch])
+        msgs, notes = backend.step([clone(e) for e in batch])
         out.append(([m.key() for m in msgs], [n.key() for n in notes]))
     rows = [r.key() for r in backend.read_rows(range(backend.n_rows))]
     return out, rows, backend.counters()

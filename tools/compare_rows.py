@@ -5,13 +5,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests")); sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 from ra_b200 import abi
 from oracle_lib import Oracle
-import make_golden, trace_gen
+import make_golden
+from ra_suite import clone
 rows_file, name = sys.argv[1], sys.argv[2]
 g, m, steps, seed, knobs, cfg = make_golden.TRACES[name]
 batches = make_golden.unpack_batches(open(os.path.join(ROOT, "tests", "golden", name + ".events.z"), "rb").read())
 o = Oracle(g, m, **cfg)
 for b in batches:
-    o.step([trace_gen.copy_ev(e) for e in b])
+    o.step([clone(e) for e in b])
 want = o.read_rows(range(o.n_rows))
 raw = open(rows_file, "rb").read()
 sz = C.sizeof(abi.RaRowState)
