@@ -566,7 +566,15 @@ size_t ra_wal_batch_to_events(const ra_wal_writer* writers, size_t n_writers, ui
 typedef struct ra_hostsim ra_hostsim;
 int  ra_hostsim_create(ra_engine* e, ra_hostsim** out);
 /* the same over K engines holding disjoint sets of groups (partition p runs the model with seed + p): one
-   host thread keeps all of them busy through ra_engine_submit_host / ra_engine_collect */
+   host thread keeps all of them busy through ra_engine_submit_host / ra_engine_collect.
+   Both create calls read these environment variables; none of them changes the rows a run leaves:
+     RA_HOSTSIM_THREADS     host-model threads in total (default: the hardware threads, at most 16); each takes a
+                            slice of a partition's rows, and a partition under 4096 rows runs on one thread
+     RA_HOSTSIM_DRIVERS     driver threads that share out the partitions, each with threads / drivers model threads
+                            (default 1, at most K)
+     RA_HOSTSIM_COMPACT     0: notes travel as 32-byte ra_note records; otherwise (default) as ra_note16 units
+     RA_HOSTSIM_NOTE_SLOTS  32-byte note slots per row that a partition's note buffer starts with (default 6); a
+                            call whose notes do not fit grows the buffer and fetches them (ra_engine_fetch_output) */
 int  ra_hostsim_create_multi(ra_engine* const* engines, uint32_t n, ra_hostsim** out);
 void ra_hostsim_destroy(ra_hostsim* s);
 /* bootstrap != 0: first send election_timeout to slot 0 of every group (ra:trigger_election) */

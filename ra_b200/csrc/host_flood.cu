@@ -91,6 +91,11 @@ extern "C" int ra_hostsim_create_multi(ra_engine* const* engines, uint32_t n, ra
     if (!engines || !n || !out) return RA_E_INVAL;
     ra_hostsim* s = new ra_hostsim();
     s->parts.resize(n);
+    // a flood row emits <= 2 WAL_APPEND + COMMIT + APPLY + STATUS notes per step in steady state; the rare step that
+    // needs more is fetched again with a bigger buffer (RA_E_CAPACITY loses nothing).  RA_HOSTSIM_NOTE_SLOTS starts
+    // the buffers smaller (or larger), e.g. 1 so that the steady flood itself needs that second fetch.
+    const char* se = getenv("RA_HOSTSIM_NOTE_SLOTS");
+    const size_t slots = se && atoi(se) > 0 ? (size_t)atoi(se) : 6;
     u32 max_rows = 0;
     for (u32 i = 0; i < n; i++) {
         Part& p = s->parts[i];
@@ -98,9 +103,7 @@ extern "C" int ra_hostsim_create_multi(ra_engine* const* engines, uint32_t n, ra
         if (!engines[i] || ra_engine_get_cfg(engines[i], &cfg) != RA_OK || !cfg.route_on_device) { ra_hostsim_destroy(s); return RA_E_INVAL; }
         p.e = engines[i]; p.groups = cfg.n_groups; p.members = cfg.n_members; p.rows = p.groups * p.members;
         p.role.assign(p.rows, RA_FOLLOWER); p.idle.assign(p.rows, 0);
-        // a flood row emits <= 2 WAL_APPEND + COMMIT + APPLY + STATUS notes per step in steady state; the rare
-        // step that needs more is fetched again with a bigger buffer (RA_E_CAPACITY loses nothing)
-        p.ev_cap = (size_t)p.rows * RA_LOCAL_CAP; p.msgs_cap = 1024; p.notes_cap = (size_t)p.rows * 6;
+        p.ev_cap = (size_t)p.rows * RA_LOCAL_CAP; p.msgs_cap = 1024; p.notes_cap = (size_t)p.rows * slots;
         p.ev = (ra_host_event*)ra_engine_alloc_host(p.ev_cap * sizeof(ra_host_event));
         p.msgs = (ra_event*)ra_engine_alloc_host(p.msgs_cap * sizeof(ra_event));
         p.notes = (ra_note*)ra_engine_alloc_host(p.notes_cap * sizeof(ra_note));
@@ -249,15 +252,24 @@ static void model(Driver* s, Part* p, size_t n_notes, u32 cmds, u32 permille, u6
 // capacity of a partition's note buffer in the units of its note format (a 32-byte slot holds two 16-byte units)
 static inline size_t note_cap_of(const Part& p) { return p.last_c.empty() ? p.notes_cap : 2 * p.notes_cap; }
 
+// extension entries of the call a partition collected (or fetched) last; the plain format has none (nor has the host
+// emulation of tests/emu/, which has the plain format only)
+static inline size_t ext_count(const Part& p)
+{
+#ifndef RA_NO_CUDA
+    if (!p.last_c.empty()) return ra_engine_last_ext_count(p.e);
+#endif
+    return 0;
+}
+
 // collect a partition's call; a note buffer that turned out too small is grown and the outputs fetched again
 static int collect_part(Driver* s, Part* p, size_t* nn)
 {
     size_t nm = 0;
     int rc = ra_engine_collect(p->e, &nm, nn);
-#ifndef RA_NO_CUDA
     if (rc == RA_E_CAPACITY) {
         // 32-byte slots the outputs need (compact: n_notes units + 2 per extension entry, two units to a slot)
-        const size_t need = p->last_c.empty() ? *nn : (*nn + 2 * ra_engine_last_ext_count(p->e) + 1) / 2;
+        const size_t need = p->last_c.empty() ? *nn : (*nn + 2 * ext_count(*p) + 1) / 2;
         if (need + need / 8 > p->notes_cap) {
             ra_engine_free_host(p->notes);
             p->notes_cap = need * 2 + 1024;
@@ -271,15 +283,12 @@ static int collect_part(Driver* s, Part* p, size_t* nn)
         if (!p->notes || !p->msgs) return RA_E_NOMEM;
         rc = ra_engine_fetch_output(p->e, p->msgs, p->msgs_cap, &nm, p->notes, note_cap_of(*p), nn);
     }
-#endif
     if (rc) return rc;
-#ifndef RA_NO_CUDA
     if (!p->last_c.empty()) {
-        p->n_ext = ra_engine_last_ext_count(p->e);
+        p->n_ext = ext_count(*p);
         s->d2h += (*nn + 2 * p->n_ext) * sizeof(ra_note16) + nm * sizeof(ra_event);
         return RA_OK;
     }
-#endif
     s->d2h += *nn * sizeof(ra_note) + nm * sizeof(ra_event);
     return RA_OK;
 }
