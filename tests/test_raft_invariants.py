@@ -619,7 +619,7 @@ def test_closed_loop_with_restarts_across_the_narrow_limit(backend, base, term, 
 
 
 @pytest.mark.parametrize("backend", CPU_BACKENDS)
-@pytest.mark.parametrize("m", [3, 5, 7])
+@pytest.mark.parametrize("m", [1, 2, 3, 5, 6, 7])
 def test_closed_loop_with_restarts_routed(backend, m, monkeypatch):
     b = _backend(backend, 12, m, monkeypatch, route_on_device=True)
     run_closed_loop(b, 300, 500 + m)
@@ -629,7 +629,8 @@ def test_closed_loop_with_restarts_routed(backend, m, monkeypatch):
 # have their own hot kernel in both passes; unrouted, only M = 5 has one (TR_HOST); every other M runs the runtime-M
 # kernel, which has no 32-bit pass -- so RA_STEP_WIDE only matters for the first two.
 CLOSED_GPU = ([(m, g, True, w) for m, g in ((3, 512), (5, 384), (7, 256)) for w in WIDTHS]
-              + [(5, 384, False, w) for w in WIDTHS] + [(4, 384, False, None), (8, 256, False, None)])
+              + [(5, 384, False, w) for w in WIDTHS] + [(4, 384, False, None), (8, 256, False, None)]
+              + [(2, 512, True, None), (6, 256, True, None)])
 
 
 @pytest.mark.gpu

@@ -170,7 +170,8 @@ def _emu_coverage(transport, m):
         assert ns["rows_narrow"] > 0 and ns["rows_wide"] > 0 and ns["records_refused"] > 0, ns
 
 
-EMU_SHAPES = [(2, 5), (3, 5), (2, 3), (3, 7), (8, 5), (4, 4), (5, 8), (8, 3)]      # (shards, members)
+# (shards, members); (3, 2): fewer members than shards
+EMU_SHAPES = [(2, 5), (3, 5), (2, 3), (3, 7), (8, 5), (4, 4), (5, 8), (8, 3), (3, 2), (2, 6)]
 
 
 @pytest.mark.parametrize("transport", TRANSPORTS)
@@ -218,7 +219,7 @@ def _engine_sharded(transports, n, G, m, monkeypatch, **cfg):
     return out
 
 
-GPU_SHAPES = [(2, 5), (8, 5), (5, 5), (3, 7), (4, 3), (8, 8)]          # (5, 5): every member on its own shard
+GPU_SHAPES = [(2, 5), (8, 5), (5, 5), (3, 7), (4, 3), (8, 8), (3, 2), (2, 6)]   # (5, 5): every member on its own shard
 
 
 @pytest.mark.gpu
