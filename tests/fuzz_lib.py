@@ -209,6 +209,20 @@ OFFSETS = [(0, 0), (LIM - 9, 0), (0, LIM - 4), (LIM - 9, LIM - 4), (LIM + 5, 3),
            ((1 << 32) - 9, (1 << 32) - 4), ((1 << 40) + 1, 1 << 35)]
 
 
+# the settings of the crafted-case tables (tests/test_quorum_table.py, tests/test_log_view_table.py), by name:
+# (engine config, RA_STEP_WIDE, (index shift, term shift) or None, leaders' replies stay in the hot kernel)
+TABLE_SETTINGS = {
+    "routed-32bit": (dict(route_on_device=True), "0", None, True),
+    "routed-64bit": (dict(route_on_device=True), "1", None, True),
+    "host": (dict(route_on_device=False), "0", None, True),
+    "pure": (dict(pure=True), "0", None, False),
+    "past2^30-32bit": (dict(route_on_device=True), "0", (LIM + 5, LIM + 3), False),
+    "past2^30-64bit": (dict(route_on_device=True), "1", (LIM + 5, LIM + 3), True),
+    "past2^32-32bit": (dict(route_on_device=True), "0", ((1 << 32) + 5, (1 << 32) + 3), False),
+    "past2^32-64bit": (dict(route_on_device=True), "1", ((1 << 32) + 5, (1 << 32) + 3), True),
+}
+
+
 def shift_state(s: abi.RaRowState, di: int, dt: int, m: int) -> None:
     for f in ("commit_index", "last_applied", "first_index", "last_index", "last_written_index", "snapshot_index",
               "cond_reply_next_index", "cond_reply_last_index"):

@@ -27,7 +27,7 @@ import random
 import pytest
 
 from emu_lib import Emu
-from fuzz_lib import compare, observe, shift_event, shift_state
+from fuzz_lib import TABLE_SETTINGS as SETTINGS, compare, observe, shift_event, shift_state
 from oracle_lib import Oracle
 from ra_b200 import abi
 from ra_suite import clone, make_backend
@@ -35,19 +35,8 @@ from ra_suite import clone, make_backend
 T, C0 = 7, 10                                   # current term and commit_index of the crafted rows
 VALS = [C0 - 1, C0, C0 + 1, C0 + 2]             # match indexes, last_written, reply indexes
 LAST = C0 + 2                                   # a leader's last index
-LIM = 1 << 30
 
-# name: (engine config, RA_STEP_WIDE, (index shift, term shift) or None, leaders' replies stay in the hot kernel)
-SETTINGS = {
-    "routed-32bit": (dict(route_on_device=True), "0", None, True),
-    "routed-64bit": (dict(route_on_device=True), "1", None, True),
-    "host": (dict(route_on_device=False), "0", None, True),
-    "pure": (dict(pure=True), "0", None, False),
-    "past2^30-32bit": (dict(route_on_device=True), "0", (LIM + 5, LIM + 3), False),
-    "past2^30-64bit": (dict(route_on_device=True), "1", (LIM + 5, LIM + 3), True),
-    "past2^32-32bit": (dict(route_on_device=True), "0", ((1 << 32) + 5, (1 << 32) + 3), False),
-    "past2^32-64bit": (dict(route_on_device=True), "1", ((1 << 32) + 5, (1 << 32) + 3), True),
-}
+# SETTINGS, name: (engine config, RA_STEP_WIDE, (index shift, term shift) or None, leaders' replies stay in the hot kernel)
 MEMBERS = list(range(1, abi.RA_MAX_MEMBERS + 1))
 
 
