@@ -34,12 +34,7 @@
 #define MINB_NARROW 5                       // the narrow pass (32-bit index arithmetic) fits 96 registers without
 #endif                                      // spilling at 5 CTAs/SM; at 6 it spills and is slower (DESIGN.md §4)
 #define TILE_BYTES (RT * 64)
-#define RA_BAR_WORDS 64                       // barrier flag words behind mbox_cnt[b] (one per source shard)
 #define WARPS (CTA_T / 32)
-// Cols::counters: [0..7] ra_counters' aggregate fields, [8..135] stall histogram (role x type),
-// [136..142] the reference's per-path counters in the order of Member::c_ref (CR_*)
-#define RA_N_COUNTERS (8 + 8 * 16 + 8)
-#define RA_CNT_REF 136
 
 // ---- TMA (cp.async.bulk) + mbarrier, sm_90a ------------------------------------------------
 __device__ __forceinline__ u32 smem_u32(const void* p) { return (u32)__cvta_generic_to_shared(p); }
@@ -281,49 +276,13 @@ __global__ void read_query_kernel(const Cols C, ra_query_state* out, u32 n)
     if (i < n) read_query_row(C, out[i]);
 }
 
-// The two record forms of a host batch: which types each may carry, and how one record is stored as the k-th local
-// record of its row, returning its loc_n size bits for k = 0 (8 + k: tail, 12 + k: not short).
-// 64-byte ra_event: any event type, stored as it is.
-__device__ __forceinline__ bool ingest_type_ok(const ra_event& ev)
-{
-    return ev.type <= RA_EV_CONSISTENT_QUERY && ev.type != RA_EV_NONE;
-}
-__device__ __forceinline__ u32 ingest_store(const Cols& C, u32 k, u32 row, const ra_event& ev)
-{
-    const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev));
-    return ((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12);
-}
-// 32-byte ra_host_event: host-origin types only (no RPC), every record RS_PLAIN
-__device__ __forceinline__ bool ingest_type_ok(const ra_host_event& ev)
-{
-    const u32 t = ev.type;
-    return t == RA_EV_WRITTEN || t == RA_EV_COMMAND || t == RA_EV_ELECTION_TIMEOUT || t == RA_EV_AWAIT_COND_TIMEOUT ||
-           t == RA_EV_PIPELINE_RPCS || t == RA_EV_TICK || t == RA_EV_CONSISTENT_QUERY;
-}
-__device__ __forceinline__ u32 ingest_store(const Cols& C, u32 k, u32 row, const ra_host_event& ev)
-{
-    const ulonglong2* src = reinterpret_cast<const ulonglong2*>(&ev);
-    const ulonglong2 h = src[0], t = src[1];                   // {row | type<<32 | flags<<40 | n<<48, term}, {a, b}
-    const u32 type = (u32)(h.x >> 32) & 0xffu, flags = (u32)(h.x >> 40) & 0xffu, nn = (u32)(h.x >> 48);
-    return put_local(C.loc, C.tiles, k, row, type, flags, nn, h.y, t.x, t.y) << 12;
-}
-
-// flat host batch -> per-row local slots.  err[0]: 1 = ungrouped, 2 = too many for a row, 3 = bad row or type
+// flat host batch -> per-row local slots, one event per thread (raft_row.cuh: ingest_event)
 template <typename EV>
 __global__ void ingest_kernel(const Cols C, const EV* ev, u32 n, u32* err, const u32* sticky)
 {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || *sticky) return;
-    const u32 row = ev[i].row;
-    if (row >= C.rows || !ingest_type_ok(ev[i])) { atomicMax(err, 3u); return; }
-    if (i > 0 && ev[i - 1].row == row) return;                 // not the head of its run
-    u32 len = 1;
-    while (i + len < n && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
-    if (len > RA_LOCAL_CAP) { atomicMax(err, 2u); return; }
-    if (atomicCAS(&C.loc_n[row], 0u, len) != 0u) { atomicMax(err, 1u); return; }
-    u32 size = 0;
-    for (u32 k = 0; k < len; k++) size |= ingest_store(C, k, row, ev[i + k]) << k;
-    if (size) atomicOr(&C.loc_n[row], size);
+    ingest_event(C, ev, n, i, err);
 }
 
 // records that other shards sent to members of this engine -> mailbox planes of the next step.
@@ -698,18 +657,15 @@ static const StepSpec& pick_step_kernel(u32 members, int tr, bool faults)
 
 extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
 {
-    if (!cfg || !out || cfg->n_members < 1 || cfg->n_members > RA_MAX_MEMBERS || cfg->n_groups == 0) return RA_E_INVAL;
-    if ((u64)cfg->n_groups * cfg->n_members > 0x7fffffffull) return RA_E_INVAL;
-    if (cfg->n_shards > 1 && (!cfg->route_on_device || cfg->shard >= cfg->n_shards || cfg->n_shards > 64)) return RA_E_INVAL;
-    if (cfg->note_cap && (cfg->note_cap < RA_NOTE_RESERVE + 2 || cfg->note_cap > RA_NOTE_CAP)) return RA_E_INVAL;
+    ra_engine_cfg c;
+    int narrow_mode;
+    if (!out || cfg_resolve(cfg, c, narrow_mode) != RA_OK) return RA_E_INVAL;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || cfg->device >= ndev) return RA_E_NODEVICE;
     ra_engine* e = (ra_engine*)calloc(1, sizeof(ra_engine));
     if (!e) return RA_E_NOMEM;
-    e->cfg = *cfg;
-    { const char* w = getenv("RA_STEP_WIDE"); e->narrow_mode = !(w && *w) ? 0 : (*w == '0' ? 1 : 2); e->narrow = e->narrow_mode != 2; }
-    if (e->cfg.max_pipeline_count == 0) e->cfg.max_pipeline_count = 4096;
-    if (e->cfg.max_aer_batch == 0) e->cfg.max_aer_batch = 128;
+    e->cfg = c;
+    e->narrow_mode = narrow_mode;
     int rc = RA_OK;
     cudaError_t ce;
     if ((ce = cudaSetDevice(cfg->device)) != cudaSuccess) { rc = fail(e, ce, "cudaSetDevice"); goto bad; }
@@ -724,35 +680,11 @@ extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
         cudaEventCreateWithFlags(&q.h2d_done, cudaEventDisableTiming);
         cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming);
     }
+    if ((rc = cols_init(e->C, e->cfg, [e](auto*& p, size_t n) { return dalloc(e, &p, n); })) != RA_OK) goto bad;
     {
         Cols& C = e->C;
-        const size_t R = (size_t)cfg->n_groups * cfg->n_members, M = cfg->n_members;
-        C.rows = (u32)R; C.groups = cfg->n_groups; C.members = cfg->n_members;
-        C.groups_inv = cfg->n_groups > 1 ? (u32)(0x100000000ull / cfg->n_groups) : 0xFFFFFFFFu;
-        C.max_pipeline = e->cfg.max_pipeline_count; C.max_batch = e->cfg.max_aer_batch;
-        C.routed = cfg->route_on_device ? 1 : 0; C.pure = cfg->pure ? 1 : 0;
-        C.note_cap = cfg->note_cap ? cfg->note_cap : RA_NOTE_CAP;
-        C.n_shards = cfg->n_shards > 1 ? cfg->n_shards : 1; C.shard = cfg->n_shards > 1 ? cfg->shard : 0;
-        C.outbox = nullptr; C.out_cnt = nullptr; C.out_cap = 0;
-        C.peer_mode = 0;
-        for (int b = 0; b < 2; b++) for (int k = 0; k < 8; k++) { C.peer_mbox[b][k] = nullptr; C.peer_cnt[b][k] = nullptr; }
+        const size_t R = C.rows;
 #define DA(p, n) if ((rc = dalloc(e, &(p), (n))) != RA_OK) goto bad
-        DA(C.tc, R); DA(C.lg, R); DA(C.lw, R); DA(C.ap, R); DA(C.sn, R); DA(C.tk, R); DA(C.fm, R);
-        DA(C.cd, 2 * R); DA(C.pnm, M * R); DA(C.pcs, M * R); DA(C.run, RA_MAX_RUNS * R); DA(C.lrs, R);
-        DA(C.qi, R); DA(C.qa, R); DA(C.pqi, M * R); DA(C.q_used, 4); DA(C.wc, R); DA(C.wf, R);
-        C.tiles = (u32)((R + RT - 1) / RT);
-        const size_t PW = (size_t)C.tiles * 4 * RT;             // 16-byte words per tiled plane
-        DA(C.loc, (size_t)RA_LOCAL_CAP * PW); DA(C.loc_n, R);
-        DA(C.onote, (size_t)RA_NOTE_CAP * R); DA(C.out_n, R + 1); DA(C.counters, RA_N_COUNTERS);   // out_n[R] stays 0: the scan's total
-        if (C.routed) {
-            // + RA_BAR_WORDS: the peer transport's step barrier flags live behind the counts of buffer 0,
-            // so they are covered by the IPC mapping the peers already have
-            for (int b = 0; b < 2; b++) { DA(C.mbox[b], M * RA_MBOX_DEPTH * PW); DA(C.mbox_cnt[b], R + RA_BAR_WORDS); }
-            DA(C.omsg, (size_t)RA_MSG_CAP * (C.pure ? R : 1));
-        } else {
-            C.mbox[0] = C.mbox[1] = nullptr; C.mbox_cnt[0] = C.mbox_cnt[1] = nullptr;
-            DA(C.omsg, (size_t)RA_MSG_CAP * R);
-        }
         DA(e->d_offs, R + 1); DA(e->d_err, 4); DA(e->d_next, R + 1); DA(e->d_xoffs, R + 1);
         DA(e->d_stall, R); DA(e->d_stall_cnt, 4);
 #undef DA
@@ -801,9 +733,8 @@ static int ensure(ra_engine* e, T** p, size_t* cap, size_t need)
 template <typename T>
 static int stage_rows(ra_engine* e, T* rows, size_t n, void (*kernel)(Cols, T*, u32))
 {
-    if (!e || (!rows && n)) return RA_E_INVAL;
+    if (!e || !rows_ok(e->C, rows, n)) return RA_E_INVAL;
     if (n == 0) return RA_OK;
-    for (size_t i = 0; i < n; i++) if (rows[i].row >= e->C.rows) return RA_E_INVAL;
     CK(cudaSetDevice(e->cfg.device));
     const size_t bytes = n * sizeof(T);
     int rc = ensure(e, &e->d_stage, &e->d_stage_cap, bytes); if (rc) return rc;
@@ -817,15 +748,8 @@ static int stage_rows(ra_engine* e, T* rows, size_t n, void (*kernel)(Cols, T*, 
 
 extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
 {
-    if (!e || (!rows && n)) return RA_E_INVAL;
-    for (size_t i = 0; i < n; i++)
-        if (rows[i].row >= e->C.rows || rows[i].n_members != e->C.members || !ra_row_state_valid(&rows[i])) return RA_E_INVAL;
-    if (e->narrow_mode == 0 && n * 2 >= e->C.rows) {       // a bulk load: which hot kernel suits this engine?
-        size_t wide = 0;
-        for (size_t i = 0; i < n; i++) wide += row_state_is_wide(rows[i], e->C.members) ? 1 : 0;
-        e->narrow = wide * 2 < n;
-    }
-    return stage_rows(e, rows, n, load_rows_kernel);
+    const int rc = e ? load_rows_check(e->C, rows, n, e->narrow_mode, e->narrow) : RA_E_INVAL;
+    return rc ? rc : stage_rows(e, rows, n, load_rows_kernel);
 }
 extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n)
 { return stage_rows(e, rows, n, read_rows_kernel); }
@@ -859,9 +783,8 @@ static int launch_step(ra_engine* e, const FloodArgs& F)
     }
     const u32 grid = (e->C.tiles + WARPS - 1) / WARPS;
     u32* cnt = e->d_stall_cnt + (e->steps & 1), *cnt_next = e->d_stall_cnt + ((e->steps + 1) & 1);
-    const int tr = !e->C.routed ? TR_HOST : (e->C.n_shards > 1 ? (e->C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
     const bool faults = (F.drop | F.withhold | F.part) != 0;     // fault injection: its own specialisations
-    const StepSpec& s = pick_step_kernel(e->C.members, tr, faults);
+    const StepSpec& s = pick_step_kernel(e->C.members, step_transport(e->C), faults);
     // 32-bit index arithmetic where the specialisation has it (exact: rows or records that do not fit stall to the
     // 64-bit general kernel); RA_STEP_WIDE=1 in the environment keeps the 64-bit hot kernel
     const bool narrow = e->narrow && s.narrow;
@@ -932,7 +855,7 @@ static int submit_impl(ra_engine* e, const EvSeg* segs, size_t n_segs, bool host
 {
     if (!e || (!segs && n_segs) || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
     size_t n_ev = 0;
-    for (size_t k = 0; k < n_segs; k++) { if (!segs[k].p && segs[k].n) return RA_E_INVAL; n_ev += segs[k].n; }
+    for (size_t k = 0; k < n_segs; k++) n_ev += segs[k].n;     // (the entry points checked each piece)
     if (n_ev > 0x7fffffffull) return RA_E_INVAL;
     if (e->out_pending) return RA_E_CAPACITY;                     // ra_engine_fetch_output first
     IoSlot& q = e->io[e->io_head % RA_IO_SLOTS];
@@ -1052,8 +975,8 @@ extern "C" int ra_engine_submit_host(ra_engine* e, const ra_host_event* ev, size
 extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg* segs, size_t n_segs,
                                           ra_event* msgs, size_t msgs_cap, ra_note* notes, size_t notes_cap)
 {
-    if (n_segs > 256 || (!segs && n_segs)) return RA_E_INVAL;
-    EvSeg s[256];
+    if (!host_segs_ok(segs, n_segs)) return RA_E_INVAL;
+    EvSeg s[RA_MAX_SEGS];
     for (size_t k = 0; k < n_segs; k++) { s[k].p = segs[k].ev; s[k].n = segs[k].n; }
     return submit_impl(e, s, n_segs, true, msgs, msgs_cap, notes, notes_cap);
 }
@@ -1138,15 +1061,13 @@ extern "C" int ra_engine_flood(ra_engine* e, uint32_t n_steps, uint32_t cmds_per
 extern "C" int ra_engine_flood_faults(ra_engine* e, uint32_t n_steps, uint32_t cmds_per_step,
                                       uint32_t election_permille, uint64_t seed, const ra_flood_faults* ff)
 {
-    if (!e || !e->C.routed) return RA_E_INVAL;
-    if (ff && ff->partition_permille && !ff->partition_steps) return RA_E_INVAL;
+    FloodArgs F;
+    const int rc0 = e ? flood_args(e->C, ff, cmds_per_step, election_permille, seed, F) : RA_E_INVAL;
+    if (rc0) return rc0;
     CK(cudaSetDevice(e->cfg.device));
     CK(cudaEventRecord(e->ev0, e->stream));
     for (u32 t = 0; t < n_steps; t++) {
-        FloodArgs F; memset(&F, 0, sizeof F);
-        F.on = 1; F.cmds = cmds_per_step; F.permille = election_permille;
-        if (ff) { F.drop = ff->drop_permille; F.withhold = ff->withhold_permille; F.part = ff->partition_permille; F.part_len = ff->partition_steps; }
-        F.seed = seed; F.step = e->step_no + t;
+        F.step = e->step_no + t;
         int rc = launch_step(e, F);
         if (rc) return rc;
         if (e->flood_barrier && e->C.peer_mode) {               // lock step with the other shards, no host in the loop
@@ -1179,7 +1100,8 @@ extern "C" int ra_engine_stall_histogram(ra_engine* e, uint64_t* out128)
 {
     if (!e || !out128) return RA_E_INVAL;
     CK(cudaSetDevice(e->cfg.device));
-    CK(cudaMemcpyAsync(out128, e->C.counters + 8, 128 * sizeof(u64), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(out128, e->C.counters + RA_CNT_STALL, (RA_CNT_REF - RA_CNT_STALL) * sizeof(u64),
+                       cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return RA_OK;
 }
@@ -1196,15 +1118,11 @@ extern "C" int ra_engine_set_stream(ra_engine* e, void* cuda_stream)
 }
 
 extern "C" int ra_engine_set_outbox(ra_engine* e, void* outbox, uint32_t* counts, uint32_t cap)
-{
-    if (!e || e->C.n_shards < 2 || !outbox || !counts || !cap) return RA_E_INVAL;
-    e->C.outbox = (ra_event*)outbox; e->C.out_cnt = counts; e->C.out_cap = cap;
-    return RA_OK;
-}
+{ return e ? cols_set_outbox(e->C, outbox, counts, cap) : RA_E_INVAL; }
 
 extern "C" int ra_engine_deliver(ra_engine* e, const void* inbox, const uint32_t* counts, uint32_t cap)
 {
-    if (!e || e->C.n_shards < 2 || !inbox || !counts || !cap) return RA_E_INVAL;
+    if (!e || !deliver_args_ok(e->C, inbox, counts, cap)) return RA_E_INVAL;
     CK(cudaSetDevice(e->cfg.device));
     // e->cur is the buffer the next step reads: the one the last step's senders wrote into
     dim3 grid(nblocks(cap, 256) < 512 ? nblocks(cap, 256) : 512, e->C.n_shards);
@@ -1214,23 +1132,10 @@ extern "C" int ra_engine_deliver(ra_engine* e, const void* inbox, const uint32_t
 }
 
 extern "C" int ra_engine_peer_get(ra_engine* e, ra_peer_ptrs* out)
-{
-    if (!e || !out || !e->C.routed) return RA_E_INVAL;
-    for (int b = 0; b < 2; b++) { out->mbox[b] = e->C.mbox[b]; out->mbox_cnt[b] = e->C.mbox_cnt[b]; }
-    return RA_OK;
-}
+{ return e ? cols_peer_get(e->C, out) : RA_E_INVAL; }
 
 extern "C" int ra_engine_peer_set(ra_engine* e, uint32_t shard, const ra_peer_ptrs* p)
-{
-    if (!e || !p || e->C.n_shards < 2 || e->C.n_shards > 8 || shard >= e->C.n_shards) return RA_E_INVAL;
-    Cols& C = e->C;
-    for (int b = 0; b < 2; b++) { C.peer_mbox[b][shard] = (ulonglong2*)p->mbox[b]; C.peer_cnt[b][shard] = (u64*)p->mbox_cnt[b]; }
-    for (int b = 0; b < 2; b++) { C.peer_mbox[b][C.shard] = C.mbox[b]; C.peer_cnt[b][C.shard] = C.mbox_cnt[b]; }
-    bool all = true;
-    for (u32 k = 0; k < C.n_shards; k++) all = all && C.peer_mbox[0][k] && C.peer_mbox[1][k] && C.peer_cnt[0][k] && C.peer_cnt[1][k];
-    C.peer_mode = all ? 1 : 0;
-    return RA_OK;
-}
+{ return e ? cols_peer_set(e->C, shard, p) : RA_E_INVAL; }
 
 extern "C" int ra_engine_peer_barrier(ra_engine* e)
 {
@@ -1315,11 +1220,6 @@ extern "C" int ra_engine_counters(ra_engine* e, ra_counters* out)
     u64 h[RA_N_COUNTERS];
     CK(cudaMemcpyAsync(h, e->C.counters, sizeof h, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    out->aer_received_follower = h[RA_CNT_REF + 0]; out->aer_received_follower_empty = h[RA_CNT_REF + 1];
-    out->aer_replies_success = h[RA_CNT_REF + 2]; out->aer_replies_failed = h[RA_CNT_REF + 3];
-    out->elections = h[RA_CNT_REF + 4]; out->pre_vote_elections = h[RA_CNT_REF + 5];
-    out->term_and_voted_for_updates = h[RA_CNT_REF + 6];
-    out->events = h[0]; out->commits = h[1]; out->applied = h[2]; out->msgs_out = h[3];
-    out->msgs_dropped = h[4]; out->elections_won = h[5]; out->fatal_rows = h[6]; out->steps = e->steps;
+    counters_unpack(h, e->steps, out);
     return RA_OK;
 }

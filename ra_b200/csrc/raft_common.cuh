@@ -107,7 +107,7 @@ struct Cols {
     ra_event* omsg;     // [k][rows] outgoing RPC records (non-routed)
     ra_note*  onote;    // [k][rows]
     u32*      out_n;    // [rows] msgs | notes << 16
-    u64*      counters; // ra_counters as 8 x u64, then [8 + role*16 + type]: events that left the fast kernel
+    u64*      counters; // [RA_N_COUNTERS]: ra_counters' fields, the stall histogram, the reference's counters (raft_row.cuh)
     u32*      abort;    // != 0: a host batch was rejected (ra_engine_submit); the step kernels do nothing until the host has cleaned up
     u32 rows, groups, members;
     u32 groups_inv;        // floor(2^32 / groups)

@@ -140,7 +140,7 @@ raft_step_kernel(const __grid_constant__ Cols C, const int cur, const FloodArgs 
             else if (!fits || !note_budget_ok(m) || C.pure || !fast_event<MM>(m, e)) {
                 stalled = true;                                 // planes are consumed in bit order:
                 rem = mine & ~(((mask_t)1 << p) - 1);           // p and up are left for the general kernel
-                atomicAdd(&C.counters[8 + (m_role(m) & 7u) * 16 + (R_type(e) & 15u)], 1ull);   // diagnostics
+                atomicAdd(&C.counters[cnt_stall(m_role(m), R_type(e))], 1ull);   // diagnostics
             }
         }
         TL(if (lane == 0) {

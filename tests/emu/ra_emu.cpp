@@ -69,60 +69,28 @@ extern "C" int ra_engine_reset_empty(ra_engine* e)
 {
     if (!e) return RA_E_INVAL;
     for (u32 r = 0; r < e->C.rows; r++) reset_row(e->C, r);
-    memset(e->C.counters, 0, (8 + 8 * 16 + 8) * sizeof(u64));
+    memset(e->C.counters, 0, RA_N_COUNTERS * sizeof(u64));
     e->C.q_used[0] = 0;
     e->cur = 0; e->step_no = 0; e->steps = 0;
     e->narrow = e->narrow_mode != 2;
+    e->out_pending = 0; e->sub_n = 0; e->sub_abort = 0; e->out_held = 0;   // as the engine drops its calls in flight
     return RA_OK;
 }
 
 extern "C" int ra_engine_create(const ra_engine_cfg* cfg, ra_engine** out)
 {
-    if (!cfg || !out || cfg->n_members < 1 || cfg->n_members > RA_MAX_MEMBERS || cfg->n_groups == 0) return RA_E_INVAL;
-    if ((u64)cfg->n_groups * cfg->n_members > 0x7fffffffull) return RA_E_INVAL;
-    if (cfg->n_shards > 1 && (!cfg->route_on_device || cfg->shard >= cfg->n_shards || cfg->n_shards > 64)) return RA_E_INVAL;
+    ra_engine_cfg c;
+    int narrow_mode;
+    if (!out || cfg_resolve(cfg, c, narrow_mode) != RA_OK) return RA_E_INVAL;
     ra_engine* e = (ra_engine*)calloc(1, sizeof(ra_engine));
     if (!e) return RA_E_NOMEM;
-    e->cfg = *cfg;
-    { const char* w = getenv("RA_STEP_WIDE"); e->narrow_mode = !(w && *w) ? 0 : (*w == '0' ? 1 : 2); e->narrow = e->narrow_mode != 2; }
-    if (e->cfg.max_pipeline_count == 0) e->cfg.max_pipeline_count = 4096;
-    if (e->cfg.max_aer_batch == 0) e->cfg.max_aer_batch = 128;
-    int rc = RA_OK;
-    Cols& C = e->C;
-    const size_t R = (size_t)cfg->n_groups * cfg->n_members, M = cfg->n_members;
-    C.rows = (u32)R; C.groups = cfg->n_groups; C.members = cfg->n_members;
-    C.groups_inv = cfg->n_groups > 1 ? (u32)(0x100000000ull / cfg->n_groups) : 0xFFFFFFFFu;
-    C.max_pipeline = e->cfg.max_pipeline_count; C.max_batch = e->cfg.max_aer_batch;
-    C.routed = cfg->route_on_device ? 1 : 0; C.pure = cfg->pure ? 1 : 0;
-    C.note_cap = cfg->note_cap ? cfg->note_cap : RA_NOTE_CAP;
-    C.n_shards = cfg->n_shards > 1 ? cfg->n_shards : 1; C.shard = cfg->n_shards > 1 ? cfg->shard : 0;
-    C.outbox = nullptr; C.out_cnt = nullptr; C.out_cap = 0;
-    C.peer_mode = 0;
-    for (int b = 0; b < 2; b++) for (int k = 0; k < 8; k++) { C.peer_mbox[b][k] = nullptr; C.peer_cnt[b][k] = nullptr; }
-#define HA(p, n) if ((rc = halloc(e, &(p), (n))) != RA_OK) goto bad
-    HA(C.tc, R); HA(C.lg, R); HA(C.lw, R); HA(C.ap, R); HA(C.sn, R); HA(C.tk, R); HA(C.fm, R);
-    HA(C.cd, 2 * R); HA(C.pnm, M * R); HA(C.pcs, M * R); HA(C.run, RA_MAX_RUNS * R); HA(C.lrs, R);
-    HA(C.qi, R); HA(C.qa, R); HA(C.pqi, M * R);
-    C.tiles = (u32)((R + RT - 1) / RT);
-    {
-        const size_t PW = (size_t)C.tiles * 4 * RT;
-        HA(C.loc, (size_t)RA_LOCAL_CAP * PW); HA(C.loc_n, R);
-        HA(C.onote, (size_t)RA_NOTE_CAP * R); HA(C.out_n, R); HA(C.counters, 8 + 8 * 16 + 8); HA(C.q_used, 4); HA(C.wc, R); HA(C.wf, R);
-        if (C.routed) {
-            for (int b = 0; b < 2; b++) { HA(C.mbox[b], M * RA_MBOX_DEPTH * PW); HA(C.mbox_cnt[b], R); }
-            HA(C.omsg, (size_t)RA_MSG_CAP * (C.pure ? R : 1));
-        } else {
-            C.mbox[0] = C.mbox[1] = nullptr; C.mbox_cnt[0] = C.mbox_cnt[1] = nullptr;
-            HA(C.omsg, (size_t)RA_MSG_CAP * R);
-        }
-    }
-#undef HA
-    if ((rc = ra_engine_reset_empty(e)) != RA_OK) goto bad;
+    e->cfg = c;
+    e->narrow_mode = narrow_mode;
+    int rc = cols_init(e->C, e->cfg, [e](auto*& p, size_t n) { return halloc(e, &p, n); });
+    if (rc == RA_OK) rc = ra_engine_reset_empty(e);
+    if (rc != RA_OK) { ra_engine_destroy(e); return rc; }
     *out = e;
     return RA_OK;
-bad:
-    ra_engine_destroy(e);
-    return rc;
 }
 
 extern "C" int ra_engine_get_cfg(ra_engine* e, ra_engine_cfg* out)
@@ -134,38 +102,29 @@ extern "C" int ra_engine_get_cfg(ra_engine* e, ra_engine_cfg* out)
 
 extern "C" int ra_engine_load_rows(ra_engine* e, const ra_row_state* rows, size_t n)
 {
-    if (!e || (!rows && n)) return RA_E_INVAL;
-    for (size_t i = 0; i < n; i++)
-        if (rows[i].row >= e->C.rows || rows[i].n_members != e->C.members || !ra_row_state_valid(&rows[i])) return RA_E_INVAL;
-    if (e->narrow_mode == 0 && n * 2 >= e->C.rows) {
-        size_t wide = 0;
-        for (size_t i = 0; i < n; i++) wide += row_state_is_wide(rows[i], e->C.members) ? 1 : 0;
-        e->narrow = wide * 2 < n;
-    }
+    const int rc = e ? load_rows_check(e->C, rows, n, e->narrow_mode, e->narrow) : RA_E_INVAL;
+    if (rc) return rc;
     for (size_t i = 0; i < n; i++) load_row(e->C, rows[i]);
     return RA_OK;
 }
 
 extern "C" int ra_engine_read_rows(ra_engine* e, ra_row_state* rows, size_t n)
 {
-    if (!e || (!rows && n)) return RA_E_INVAL;
-    for (size_t i = 0; i < n; i++) if (rows[i].row >= e->C.rows) return RA_E_INVAL;
+    if (!e || !rows_ok(e->C, rows, n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) read_row(e->C, rows[i]);
     return RA_OK;
 }
 
 extern "C" int ra_engine_load_query_state(ra_engine* e, const ra_query_state* q, size_t n)
 {
-    if (!e || (!q && n)) return RA_E_INVAL;
-    for (size_t i = 0; i < n; i++) if (q[i].row >= e->C.rows) return RA_E_INVAL;
+    if (!e || !rows_ok(e->C, q, n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) load_query_row(e->C, q[i]);
     return RA_OK;
 }
 
 extern "C" int ra_engine_read_query_state(ra_engine* e, ra_query_state* q, size_t n)
 {
-    if (!e || (!q && n)) return RA_E_INVAL;
-    for (size_t i = 0; i < n; i++) if (q[i].row >= e->C.rows) return RA_E_INVAL;
+    if (!e || !rows_ok(e->C, q, n)) return RA_E_INVAL;
     for (size_t i = 0; i < n; i++) read_query_row(e->C, q[i]);
     return RA_OK;
 }
@@ -290,7 +249,7 @@ static int run_step(ra_engine* e, const FloodArgs& F)
         memset(C.out_cnt, 0, C.n_shards * sizeof(u32));
     }
     // M = 5 picks its specialisation by transport as the table k_step_kernels in engine.cu does; other M run runtime-M
-    const int tr = !C.routed ? TR_HOST : (C.n_shards > 1 ? (C.peer_mode ? TR_PEER : TR_BUCKET) : TR_LOCAL);
+    const int tr = step_transport(C);
     u32 w_tail = 0;
     for (u32 r = 0; r < C.rows; r++) {
         if ((r & (RT - 1)) == 0) w_tail = tile_sizes(C, e->cur, r);
@@ -318,15 +277,11 @@ static int run_step(ra_engine* e, const FloodArgs& F)
 }
 
 extern "C" int ra_engine_set_outbox(ra_engine* e, void* outbox, uint32_t* counts, uint32_t cap)
-{
-    if (!e || e->C.n_shards < 2 || !outbox || !counts || !cap) return RA_E_INVAL;
-    e->C.outbox = (ra_event*)outbox; e->C.out_cnt = counts; e->C.out_cap = cap;
-    return RA_OK;
-}
+{ return e ? cols_set_outbox(e->C, outbox, counts, cap) : RA_E_INVAL; }
 
 extern "C" int ra_engine_deliver(ra_engine* e, const void* inbox, const uint32_t* counts, uint32_t cap)
 {
-    if (!e || e->C.n_shards < 2 || !inbox || !counts || !cap) return RA_E_INVAL;
+    if (!e || !deliver_args_ok(e->C, inbox, counts, cap)) return RA_E_INVAL;
     const ra_event* in = (const ra_event*)inbox;
     // e->cur is the buffer the next step reads: the one the last step's senders wrote into
     for (u32 b = 0; b < e->C.n_shards; b++) {
@@ -338,23 +293,10 @@ extern "C" int ra_engine_deliver(ra_engine* e, const void* inbox, const uint32_t
 
 // the peer transport (engine.cu: ra_engine_peer_get / ra_engine_peer_set): host pointers in place of device ones
 extern "C" int ra_engine_peer_get(ra_engine* e, ra_peer_ptrs* out)
-{
-    if (!e || !out || !e->C.routed) return RA_E_INVAL;
-    for (int b = 0; b < 2; b++) { out->mbox[b] = e->C.mbox[b]; out->mbox_cnt[b] = e->C.mbox_cnt[b]; }
-    return RA_OK;
-}
+{ return e ? cols_peer_get(e->C, out) : RA_E_INVAL; }
 
 extern "C" int ra_engine_peer_set(ra_engine* e, uint32_t shard, const ra_peer_ptrs* p)
-{
-    if (!e || !p || e->C.n_shards < 2 || e->C.n_shards > 8 || shard >= e->C.n_shards) return RA_E_INVAL;
-    Cols& C = e->C;
-    for (int b = 0; b < 2; b++) { C.peer_mbox[b][shard] = (ulonglong2*)p->mbox[b]; C.peer_cnt[b][shard] = (u64*)p->mbox_cnt[b]; }
-    for (int b = 0; b < 2; b++) { C.peer_mbox[b][C.shard] = C.mbox[b]; C.peer_cnt[b][C.shard] = C.mbox_cnt[b]; }
-    bool all = true;
-    for (u32 k = 0; k < C.n_shards; k++) all = all && C.peer_mbox[0][k] && C.peer_mbox[1][k] && C.peer_cnt[0][k] && C.peer_cnt[1][k];
-    C.peer_mode = all ? 1 : 0;
-    return RA_OK;
-}
+{ return e ? cols_peer_set(e->C, shard, p) : RA_E_INVAL; }
 
 // scan + gather_out: per-row slots -> flat arrays ordered by (row, seq).  When they do not fit, nothing is
 // written and the slots stay: RA_E_CAPACITY with the sizes needed, the caller fetches again (engine.cu)
@@ -403,8 +345,9 @@ extern "C" int ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_
     return RA_OK;
 }
 
-// one call: ingest, the step, the gather (what submit_impl enqueues)
-static int eval_step(ra_engine* e, const ra_event* ev, size_t n_ev,
+// one call: ingest, the step, the gather (what submit_impl enqueues), for either record form (ra_event, ra_host_event)
+template <typename EV>
+static int eval_step(ra_engine* e, const EV* ev, size_t n_ev,
                      ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
                      ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
@@ -413,24 +356,8 @@ static int eval_step(ra_engine* e, const ra_event* ev, size_t n_ev,
     const u32 R = C.rows;
     // clear_loc_kernel, and (after a flood, whose last step wrote every row's out_n) the out_n clear of submit_impl
     for (u32 r = 0; r < R; r++) { C.loc_n[r] = 0; C.out_n[r] = 0; }
-    // ingest_kernel: flat batch -> per-row local slots
     u32 err = 0;
-    for (size_t i = 0; i < n_ev; i++) {
-        const u32 row = ev[i].row;
-        if (row >= R || ev[i].type > RA_EV_CONSISTENT_QUERY || ev[i].type == RA_EV_NONE) { if (err < 3) err = 3; continue; }
-        if (i > 0 && ev[i - 1].row == row) continue;
-        u32 len = 1;
-        while (i + len < n_ev && ev[i + len].row == row && len <= RA_LOCAL_CAP) len++;
-        if (len > RA_LOCAL_CAP) { if (err < 2) err = 2; continue; }
-        if (C.loc_n[row] != 0) { if (err < 1) err = 1; continue; }
-        C.loc_n[row] = len;
-        u32 size = 0;                                            // loc_n bits 8 + k (tail), 12 + k (not short)
-        for (u32 k = 0; k < len; k++) {
-            const u32 f = st_rec_plane(C.loc, C.tiles, k, row, ld_rec(&ev[i + k]));
-            size |= (((f & RF_TAIL) << 7) | ((f & RF_NOT_SHORT) << 12)) << k;
-        }
-        C.loc_n[row] |= size;
-    }
+    for (u32 i = 0; i < (u32)n_ev; i++) ingest_event(C, ev, (u32)n_ev, i, &err);   // ingest_kernel, one event at a time
     if (err) {
         for (u32 r = 0; r < R; r++) C.loc_n[r] = 0;
         return err == 1 ? RA_E_UNGROUPED : (err == 2 ? RA_E_CAPACITY : RA_E_INVAL);
@@ -440,47 +367,23 @@ static int eval_step(ra_engine* e, const ra_event* ev, size_t n_ev,
     return gather_out(e, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
 
-// the same for 32-byte host events: widened to 64-byte records, an RPC type rejects the batch
-static int eval_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev,
-                          ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                          ra_note* notes, size_t notes_cap, size_t* n_notes)
-{
-    if (!ev && n_ev) return RA_E_INVAL;
-    ra_event* w = (ra_event*)calloc(n_ev ? n_ev : 1, sizeof(ra_event));
-    if (!w) return RA_E_NOMEM;
-    for (size_t i = 0; i < n_ev; i++) {
-        const u32 t = ev[i].type;
-        if (!(t == RA_EV_WRITTEN || t == RA_EV_COMMAND || t == RA_EV_ELECTION_TIMEOUT || t == RA_EV_AWAIT_COND_TIMEOUT ||
-              t == RA_EV_PIPELINE_RPCS || t == RA_EV_TICK || t == RA_EV_CONSISTENT_QUERY)) { free(w); return RA_E_INVAL; }
-        w[i].row = ev[i].row; w[i].type = (uint8_t)t; w[i].from_slot = RA_NO_SLOT; w[i].flags = ev[i].flags; w[i].n = ev[i].n;
-        w[i].term = ev[i].term; w[i].a = ev[i].a; w[i].b = ev[i].b;
-    }
-    const int rc = eval_step(e, w, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
-    free(w);
-    return rc;
-}
-
 // step = submit + collect (engine.cu: step_impl): not while a submitted call waits to be collected, nor while the
 // outputs of an earlier call wait to be fetched
-extern "C" int ra_engine_step(ra_engine* e, const ra_event* ev, size_t n_ev,
-                              ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                              ra_note* notes, size_t notes_cap, size_t* n_notes)
+template <typename EV>
+static int step_impl(ra_engine* e, const EV* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
+                     ra_note* notes, size_t notes_cap, size_t* n_notes)
 {
     if (!e) return RA_E_INVAL;
     if (e->sub_n) return RA_E_BUSY;
     if (e->out_pending) return RA_E_CAPACITY;                    // ra_engine_fetch_output first
     return eval_step(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
 }
-
-extern "C" int ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev,
-                                   ra_event* msgs, size_t msgs_cap, size_t* n_msgs,
-                                   ra_note* notes, size_t notes_cap, size_t* n_notes)
-{
-    if (!e) return RA_E_INVAL;
-    if (e->sub_n) return RA_E_BUSY;
-    if (e->out_pending) return RA_E_CAPACITY;
-    return eval_step_host(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes);
-}
+extern "C" int ra_engine_step(ra_engine* e, const ra_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
+                              size_t* n_msgs, ra_note* notes, size_t notes_cap, size_t* n_notes)
+{ return step_impl(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
+extern "C" int ra_engine_step_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
+                                   size_t* n_msgs, ra_note* notes, size_t notes_cap, size_t* n_notes)
+{ return step_impl(e, ev, n_ev, msgs, msgs_cap, n_msgs, notes, notes_cap, n_notes); }
 
 extern "C" int ra_engine_flood(ra_engine* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
                                uint64_t seed)
@@ -488,13 +391,11 @@ extern "C" int ra_engine_flood(ra_engine* e, uint32_t n_steps, uint32_t cmds_per
 extern "C" int ra_engine_flood_faults(ra_engine* e, uint32_t n_steps, uint32_t cmds_per_step, uint32_t election_permille,
                                       uint64_t seed, const ra_flood_faults* ff)
 {
-    if (!e || !e->C.routed) return RA_E_INVAL;
-    if (ff && ff->partition_permille && !ff->partition_steps) return RA_E_INVAL;
+    FloodArgs F;
+    const int rc0 = e ? flood_args(e->C, ff, cmds_per_step, election_permille, seed, F) : RA_E_INVAL;
+    if (rc0) return rc0;
     for (u32 t = 0; t < n_steps; t++) {
-        FloodArgs F; memset(&F, 0, sizeof F);
-        F.on = 1; F.cmds = cmds_per_step; F.permille = election_permille;
-        if (ff) { F.drop = ff->drop_permille; F.withhold = ff->withhold_permille; F.part = ff->partition_permille; F.part_len = ff->partition_steps; }
-        F.seed = seed; F.step = e->step_no + t;
+        F.step = e->step_no + t;
         const int rc = run_step(e, F);
         if (rc) return rc;
     }
@@ -505,19 +406,14 @@ extern "C" int ra_engine_flood_faults(ra_engine* e, uint32_t n_steps, uint32_t c
 extern "C" int ra_engine_counters(ra_engine* e, ra_counters* out)
 {
     if (!e || !out) return RA_E_INVAL;
-    const u64* h = e->C.counters;
-    out->events = h[0]; out->commits = h[1]; out->applied = h[2]; out->msgs_out = h[3];
-    out->msgs_dropped = h[4]; out->elections_won = h[5]; out->fatal_rows = h[6]; out->steps = e->steps;
-    out->aer_received_follower = h[136]; out->aer_received_follower_empty = h[137]; out->aer_replies_success = h[138];
-    out->aer_replies_failed = h[139]; out->elections = h[140]; out->pre_vote_elections = h[141];
-    out->term_and_voted_for_updates = h[142];
+    counters_unpack(e->C.counters, e->steps, out);
     return RA_OK;
 }
 
 extern "C" int ra_engine_stall_histogram(ra_engine* e, uint64_t* out128)
 {
     if (!e || !out128) return RA_E_INVAL;
-    memcpy(out128, e->C.counters + 8, 128 * sizeof(u64));
+    memcpy(out128, e->C.counters + RA_CNT_STALL, (RA_CNT_REF - RA_CNT_STALL) * sizeof(u64));
     return RA_OK;
 }
 
@@ -536,8 +432,8 @@ extern "C" int ra_emu_codec_roundtrip(const ra_event* in, ra_event* out, int* ha
 /* the split-phase calls with the two-slot contract of include/ra_engine.h: the emulation evaluates a call when it is
  * submitted and hands the result over at collect.  A call submitted behind a rejected one gets the same status, one
  * submitted behind a call whose outputs did not fit gets RA_E_PENDING; neither is evaluated. */
-static int submit_call(ra_engine* m, const void* ev, size_t n_ev, bool host32, ra_event* msgs, size_t msgs_cap,
-                       ra_note* notes, size_t notes_cap)
+template <typename EV>
+static int submit_call(ra_engine* m, const EV* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap, ra_note* notes, size_t notes_cap)
 {
     if (!m || (!msgs && msgs_cap) || (!notes && notes_cap)) return RA_E_INVAL;
     if (m->out_pending && !m->out_held) return RA_E_CAPACITY;   // ra_engine_fetch_output first
@@ -545,21 +441,21 @@ static int submit_call(ra_engine* m, const void* ev, size_t n_ev, bool host32, r
     auto& s = m->sub[m->sub_n++];
     s.nm = s.nn = 0;
     if (m->sub_abort) { s.rc = m->sub_abort; return RA_OK; }
-    s.rc = host32 ? eval_step_host(m, (const ra_host_event*)ev, n_ev, msgs, msgs_cap, &s.nm, notes, notes_cap, &s.nn)
-                  : eval_step(m, (const ra_event*)ev, n_ev, msgs, msgs_cap, &s.nm, notes, notes_cap, &s.nn);
+    s.rc = eval_step(m, ev, n_ev, msgs, msgs_cap, &s.nm, notes, notes_cap, &s.nn);
     if (s.rc == RA_E_CAPACITY && m->out_pending) { m->sub_abort = RA_E_PENDING; m->out_held = 1; }
     else if (s.rc) m->sub_abort = s.rc;
     return RA_OK;
 }
 extern "C" int ra_engine_submit_host(ra_engine* e, const ra_host_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
                                      ra_note* notes, size_t notes_cap)
-{ return submit_call(e, ev, n_ev, true, msgs, msgs_cap, notes, notes_cap); }
+{ return submit_call(e, ev, n_ev, msgs, msgs_cap, notes, notes_cap); }
 extern "C" int ra_engine_submit(ra_engine* e, const ra_event* ev, size_t n_ev, ra_event* msgs, size_t msgs_cap,
                                 ra_note* notes, size_t notes_cap)
-{ return submit_call(e, ev, n_ev, false, msgs, msgs_cap, notes, notes_cap); }
+{ return submit_call(e, ev, n_ev, msgs, msgs_cap, notes, notes_cap); }
 extern "C" int ra_engine_submit_host_segs(ra_engine* e, const ra_host_event_seg* segs, size_t n_segs, ra_event* msgs,
                                           size_t msgs_cap, ra_note* notes, size_t notes_cap)
 {
+    if (!host_segs_ok(segs, n_segs)) return RA_E_INVAL;
     size_t n = 0;
     for (size_t k = 0; k < n_segs; k++) n += segs[k].n;
     ra_host_event* all = (ra_host_event*)malloc((n ? n : 1) * sizeof(ra_host_event));

@@ -101,6 +101,20 @@ def test_emu_step_input_validation():
     msgs, notes = e.step([])
     assert msgs == [] and notes == []
     assert e.counters()["events"] == 0
+    # a batch in more than 256 pieces
+    st, _ = e.submit_host_segs([[] for _ in range(257)], 64, 64)
+    assert st == abi.RA_E_INVAL
+    # reset_empty drops outputs that did not fit
+    with pytest.raises(abi.RaError) as ei:
+        e.step([abi.ev_simple(r0, abi.EV_ELECTION_TIMEOUT)], msgs_cap=0, notes_cap=0)
+    assert ei.value.status == abi.RA_E_CAPACITY
+    e.reset_empty()
+    assert e.step([]) == ([], [])
+    # note budgets outside RA_NOTE_RESERVE + 2 .. RA_NOTE_CAP
+    for cap in (abi.RA_NOTE_RESERVE + 1, abi.RA_NOTE_CAP + 1):
+        with pytest.raises(abi.RaError) as ei:
+            Emu(4, 3, note_cap=cap)
+        assert ei.value.status == abi.RA_E_INVAL
 
 
 @pytest.mark.parametrize("threads", ["1", "4"])
