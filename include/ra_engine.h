@@ -116,7 +116,10 @@ enum ra_event_type {
 typedef struct ra_event {
     uint32_t row;        /* destination member row                                  */
     uint8_t  type;       /* enum ra_event_type                                      */
-    uint8_t  from_slot;  /* sender's slot in the group, RA_NO_SLOT for host events  */
+    uint8_t  from_slot;  /* sender's slot in the group, RA_NO_SLOT for host events;
+                            0..14 or RA_NO_SLOT: a row stores leader_id and voted_for
+                            in 4 bits, so a batch with a sender in 15..254 is
+                            RA_E_INVAL (slots n_members..14 are unknown peers)      */
     uint8_t  flags;      /* RA_EVF_*                                                */
     uint8_t  _pad;
     uint16_t n;          /* entry / command count                                   */
@@ -373,7 +376,7 @@ int  ra_engine_step(ra_engine* e,
  * A call already submitted behind it (split phase, below) is not evaluated: its collect returns RA_E_PENDING and
  * no row has changed, and ra_engine_fetch_output answers RA_E_BUSY until that call is collected.  Fetch, then
  * submit that batch again.  RA_E_CAPACITY for more than RA_LOCAL_CAP events of one row, RA_E_UNGROUPED and
- * RA_E_INVAL (bad row / type) reject the whole batch: no row has changed.
+ * RA_E_INVAL (bad row / type, or a from_slot in 15..254) reject the whole batch: no row has changed.
  */
 int  ra_engine_pending_output(ra_engine* e, size_t* n_msgs, size_t* n_notes);
 int  ra_engine_fetch_output(ra_engine* e, ra_event* msgs, size_t msgs_cap, size_t* n_msgs,

@@ -1692,7 +1692,8 @@ int ra_oracle_step(ra_oracle *o, const ra_event *ev, size_t n_ev,
     /* validate grouping + capacity */
     for (size_t i = 0; i < n_ev;) {
         u32 row = ev[i].row;
-        if (row >= o->n_rows || ev[i].type > RA_EV_CONSISTENT_QUERY || ev[i].type == RA_EV_NONE) { free(seen); return RA_E_INVAL; }
+        if (row >= o->n_rows || ev[i].type > RA_EV_CONSISTENT_QUERY || ev[i].type == RA_EV_NONE ||
+            (ev[i].from_slot >= 15 && ev[i].from_slot != RA_NO_SLOT)) { free(seen); return RA_E_INVAL; }   /* sender slot: ra_engine.h */
         if (seen[row]) { free(seen); return RA_E_UNGROUPED; }
         seen[row] = 1;
         size_t j = i;

@@ -157,10 +157,11 @@ __device__ __forceinline__ void deliver_record(const Cols& C, const int buf, con
 // ---- ingest: a flat host batch -> the per-row local slots --------------------------------------
 // The two record forms of a host batch: which types each may carry, and how one record is stored as the k-th local
 // record of its row, returning its loc_n size bits for k = 0 (8 + k: tail, 12 + k: not short).
-// 64-byte ra_event: any event type, stored as it is.
+// 64-byte ra_event: any event type, stored as it is, from a slot below 15 or RA_NO_SLOT (a row keeps leader_id and
+// voted_for in 4 bits: slot 17 would be read as slot 1, include/ra_engine.h at ra_event.from_slot).
 __device__ __forceinline__ bool ingest_type_ok(const ra_event& ev)
 {
-    return ev.type <= RA_EV_CONSISTENT_QUERY && ev.type != RA_EV_NONE;
+    return ev.type <= RA_EV_CONSISTENT_QUERY && ev.type != RA_EV_NONE && (ev.from_slot < 15u || ev.from_slot == RA_NO_SLOT);
 }
 __device__ __forceinline__ u32 ingest_store(const Cols& C, u32 k, u32 row, const ra_event& ev)
 {

@@ -98,6 +98,13 @@ def test_emu_step_input_validation():
     with pytest.raises(abi.RaError) as ei:
         e.step([abi.ev_command(10_000)])
     assert ei.value.status == abi.RA_E_INVAL
+    # a sender slot a row cannot hold (15..254), through step and through submit / collect
+    bad = [abi.ev_command(r0), abi.ev_request_vote(r1, 17, 1, 0, 0)]
+    with pytest.raises(abi.RaError) as ei:
+        e.step(bad)
+    assert ei.value.status == abi.RA_E_INVAL
+    st, ticket = e.submit(bad, 64, 64)
+    assert st == abi.RA_OK and e.collect(ticket)[0] == abi.RA_E_INVAL
     msgs, notes = e.step([])
     assert msgs == [] and notes == []
     assert e.counters()["events"] == 0

@@ -397,7 +397,11 @@ def _bad_batches(G, m):
                                                abi.ev_simple(0, abi.EV_TICK)]),
             ("above RA_LOCAL_CAP", abi.RA_E_CAPACITY, [abi.ev_command(G, 1) for _ in range(abi.RA_LOCAL_CAP + 1)]),
             ("bad row", abi.RA_E_INVAL, [abi.ev_simple(1, abi.EV_TICK), abi.ev_simple(n, abi.EV_TICK)]),
-            ("bad type", abi.RA_E_INVAL, [abi.ev_simple(2, 16)])]
+            ("bad type", abi.RA_E_INVAL, [abi.ev_simple(2, 16)]),
+            ("sender slot 17", abi.RA_E_INVAL, [abi.ev_simple(1, abi.EV_TICK), abi.ev_request_vote(2, 17, 99, 0, 0)])]
+
+
+HOSTLESS = ("bad type", "sender slot 17")    # a 32-byte host record carries neither an RPC type nor a sender
 
 
 def _rejected(nif, G, m, seed):
@@ -410,11 +414,11 @@ def _rejected(nif, G, m, seed):
     for what, code, bad in _bad_batches(G, m):
         before = eng.rows_bytes()
         assert eng.step(bad) == ("error", code), what
-        if what != "bad type":                                  # (a type outside the enum is no host event either)
+        if what not in HOSTLESS:
             assert eng.step_host(bad) == ("error", code), what
         assert eng.step_host([abi.ev_aer(0, 1, 1, 0, 0, 0)]) == ("error", abi.RA_E_INVAL)   # an RPC type
         for api in ("submit", "submit_host"):
-            if api == "submit_host" and what == "bad type":
+            if api == "submit_host" and what in HOSTLESS:
                 continue
             evs = good()
             assert getattr(eng, api)(bad) == "ok" and getattr(eng, api)(evs) == "ok", what
